@@ -31,7 +31,35 @@ class OpbParams(C.Structure):
 PERSON_DTYPE = np.dtype([("score", "<f8"), ("count", "<f8"), ("peak_id", "<i4", (N_JOINTS,)),
                          ("x", "<i4", (N_JOINTS,)), ("y", "<i4", (N_JOINTS,)), ("pad", "<i4", (2,))])
 HEADER_DTYPE = np.dtype([("n_peaks", "<i4"), ("n_persons", "<i4"), ("status", "<i4"), ("n_connections", "<i4")])
-assert PERSON_DTYPE.itemsize == 240 and HEADER_DTYPE.itemsize == 16
+CROP_DTYPE = np.dtype([("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bottom", "<i4"), ("flip", "<i4"),
+                       ("reserved", "<i4")])      # opb_crop
+assert PERSON_DTYPE.itemsize == 240 and HEADER_DTYPE.itemsize == 16 and CROP_DTYPE.itemsize == 24
+
+
+def crop_table(bboxes, flips=None):
+    """(left, top, right, bottom) integer boxes (+ per-box flip flags) -> opb_crop array.  ValueError for a box that is
+    not four integers or whose canvas (bottom-top) x (right-left) is empty, so that nothing is launched for it."""
+    bboxes = list(bboxes)
+    flips = [False] * len(bboxes) if flips is None else list(flips)
+    if len(flips) != len(bboxes):
+        raise ValueError("%d boxes but %d flip flags" % (len(bboxes), len(flips)))
+    table = np.zeros(len(bboxes), CROP_DTYPE)
+    lim = np.iinfo(np.int32)
+    for i, (b, f) in enumerate(zip(bboxes, flips)):
+        try:
+            vals = tuple(b)
+        except TypeError:
+            raise ValueError("bbox %d is not a (left, top, right, bottom) tuple: %r" % (i, b))
+        if len(vals) != 4 or not all(isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+                                     for v in vals):
+            raise ValueError("bbox %d must be four integers (left, top, right, bottom): %r" % (i, b))
+        left, top, right, bottom = (int(v) for v in vals)
+        if not all(lim.min <= v <= lim.max for v in (left, top, right, bottom)):
+            raise ValueError("bbox %d does not fit int32: %r" % (i, b))
+        if right - left <= 0 or bottom - top <= 0:
+            raise ValueError("bbox %d gives an empty crop (%d x %d): %r" % (i, bottom - top, right - left, b))
+        table[i] = (left, top, right, bottom, int(bool(f)), 0)
+    return table
 
 _SIGNATURES = {
     "opb_version": (C.c_int, []),
@@ -83,6 +111,8 @@ _SIGNATURES = {
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
     "opb_keypoints_from_heatmaps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                               C.c_double, C.c_void_p, C.c_void_p]),
+    "opb_keypoints_detect_crops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                             C.c_int, C.c_double, C.c_void_p, C.c_void_p]),
     "opb_precise_add_scale_unpadded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                  C.c_int, C.c_int]),
     "opb_get_image_detail": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_void_p,
@@ -449,6 +479,27 @@ class Engine(object):
                                                   _ptr(maps) if return_maps else None))
         kps = self._keypoint_list(out, valid)
         return (kps, maps) if return_maps else kps
+
+    def keypoints_detect_crops(self, frame, crops, net_size, thresh):
+        """All crops of one BGR frame [H,W,3] -> one keypoint list per crop (opb_keypoints_detect_crops).  `crops`: an
+        opb_crop array (crop_table) or (left, top, right, bottom[, flip]) tuples; crop i gives what keypoints_detect
+        gives for flip_i(crop_image(frame, bbox_i)) with mirror=flip_i."""
+        frame = np.asarray(frame)
+        if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
+            raise ValueError("frame must be a uint8 [H, W, 3] image, got %s %s" % (frame.dtype, frame.shape))
+        frame = np.ascontiguousarray(frame)
+        if not (isinstance(crops, np.ndarray) and crops.dtype == CROP_DTYPE):
+            crops = list(crops)
+            crops = crop_table([c[:4] for c in crops], [len(c) > 4 and bool(c[4]) for c in crops])
+        crops = np.ascontiguousarray(crops)
+        n = len(crops)
+        planes = max(self.kp_channels - 1, 0)      # 0 on a pose context, which the library refuses (OPB_ERR_STATE)
+        out = np.empty((n, planes, 3), np.float64)
+        valid = np.empty((n, planes), np.int32)
+        h, w, _ = frame.shape
+        self._check(self.lib.opb_keypoints_detect_crops(self.ctx, _ptr(frame), OPB_HOST, h, w, _ptr(crops), n,
+                                                        int(net_size), float(thresh), _ptr(out), _ptr(valid)))
+        return [self._keypoint_list(o, v) for o, v in zip(out, valid)]
 
     def keypoints_from_heatmaps(self, heatmaps, thresh, mirror=False):
         """heatmaps [C,H,W] float32, background channel already dropped (opb_keypoints_from_heatmaps)."""

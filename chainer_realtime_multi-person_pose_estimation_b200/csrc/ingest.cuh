@@ -29,24 +29,80 @@ __device__ __forceinline__ void cv_linear_axis(int d, double scale, int src_n, b
   s1 = min(max(s + 1, 0), src_n - 1);
 }
 
+// One output pixel (x, y) of the INTER_LINEAR resize of an h0 x w0 BGR source read through `src(y, x, c)`.
+template <typename Src>
+__device__ __forceinline__ void cv_linear_pixel(const Src& src, int h0, int w0, int x, int y, double scale_x,
+                                                double scale_y, uint8_t* __restrict__ o) {
+  int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
+  cv_linear_axis(x, scale_x, w0, true, sx0, sx1, a0, a1);
+  cv_linear_axis(y, scale_y, h0, false, sy0, sy1, b0, b1);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int d0 = src(sy0, sx0, c) * a0 + src(sy0, sx1, c) * a1;
+    const int d1 = src(sy1, sx0, c) * a0 + src(sy1, sx1, c) * a1;
+    o[c] = static_cast<uint8_t>((((b0 * (d0 >> 4)) >> 16) + ((b1 * (d1 >> 4)) >> 16) + 2) >> 2);
+  }
+}
+
+struct DenseU8 {            // one [h0][w0][3] image
+  const uint8_t* p;
+  int w0;
+  __device__ __forceinline__ int operator()(int y, int x, int c) const { return p[(static_cast<size_t>(y) * w0 + x) * 3 + c]; }
+};
+
 // src [n][h0][w0][3] uint8 -> dst [n][h][w][3] uint8; grid (ceil(w/32), ceil(h/8), n), block (32, 8)
 __global__ void __launch_bounds__(256)
 resize_linear_u8_kernel(const uint8_t* __restrict__ src, int h0, int w0, uint8_t* __restrict__ dst, int h, int w,
                         double scale_x, double scale_y) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, n = blockIdx.z;
   if (x >= w || y >= h) return;
-  int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
-  cv_linear_axis(x, scale_x, w0, true, sx0, sx1, a0, a1);
-  cv_linear_axis(y, scale_y, h0, false, sy0, sy1, b0, b1);
-  const uint8_t* r0 = src + (static_cast<size_t>(n) * h0 + sy0) * w0 * 3;
-  const uint8_t* r1 = src + (static_cast<size_t>(n) * h0 + sy1) * w0 * 3;
-  uint8_t* o = dst + ((static_cast<size_t>(n) * h + y) * w + x) * 3;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const int d0 = r0[sx0 * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
-    const int d1 = r1[sx0 * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
-    o[c] = static_cast<uint8_t>((((b0 * (d0 >> 4)) >> 16) + ((b1 * (d1 >> 4)) >> 16) + 2) >> 2);
+  const DenseU8 s{src + static_cast<size_t>(n) * h0 * w0 * 3, w0};
+  cv_linear_pixel(s, h0, w0, x, y, scale_x, scale_y, dst + ((static_cast<size_t>(n) * h + y) * w + x) * 3);
+}
+
+// ---- face / hand crops straight from the frame (opb_keypoints_detect_crops) ----
+// One crop: the canvas of PoseDetector.crop_image (pose_detector.py:401-424) -- rows top..top+h-1, columns
+// left..left+w-1 of the frame, zero outside it -- optionally mirrored (cv2.flip(canvas, 1), hand_detector.py:29-30).
+// The same descriptor drives the ragged post-process kernels of keypoints.cuh / upsample.cuh.
+struct KpCrop {
+  long long off;        // first float of the crop's maps [planes][h][w] in the ragged workspace
+  int top, left, h, w;  // canvas origin in the frame and canvas size (= size of the crop's maps)
+  int flip;             // canvas mirrored before the net; peak positions reported in the unmirrored canvas
+  int tile0;            // first 32x8 tile of the crop in the ragged tile enumeration
+  double sx, sy;        // cv2.resize scales canvas -> net: 1 / (net / w), 1 / (net / h)
+};
+
+// The crop that owns ragged tile t: the last of crops[0..n) with tile0 <= t (tile0 ascending, crops[0].tile0 <= t).
+__device__ __forceinline__ int kp_find_crop(const KpCrop* __restrict__ crops, int n, int t) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (crops[mid].tile0 <= t) lo = mid; else hi = mid - 1;
   }
+  return lo;
+}
+
+struct CropCanvasU8 {       // crop_image(frame, bbox) (+ flip) read in place
+  const uint8_t* frame;
+  int fh, fw, top, left, w, flip;
+  __device__ __forceinline__ int operator()(int y, int x, int c) const {
+    const int fy = top + y, fx = left + (flip ? w - 1 - x : x);
+    return (fy >= 0 && fy < fh && fx >= 0 && fx < fw) ? frame[(static_cast<size_t>(fy) * fw + fx) * 3 + c] : 0;
+  }
+};
+
+// cv2.resize(flip?(crop_image(frame, crop)), (net, net)) of crops[0..n_real) into dst [gridDim.z][net][net][3]; the
+// slots n_real..gridDim.z-1 (padding of a fixed-size chunk) are zeroed.  grid (ceil(net/32), ceil(net/8), slots)
+__global__ void __launch_bounds__(256)
+crop_resize_linear_u8_kernel(const uint8_t* __restrict__ frame, int fh, int fw, const KpCrop* __restrict__ crops,
+                             int n_real, uint8_t* __restrict__ dst, int net) {
+  const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, n = blockIdx.z;
+  if (x >= net || y >= net) return;
+  uint8_t* o = dst + ((static_cast<size_t>(n) * net + y) * net + x) * 3;
+  if (n >= n_real) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
+  const KpCrop k = crops[n];
+  const CropCanvasU8 s{frame, fh, fw, k.top, k.left, k.w, k.flip};
+  cv_linear_pixel(s, k.h, k.w, x, y, k.sx, k.sy, o);
 }
 
 // ---- cv2.resize(orig_img, ..., interpolation=cv2.INTER_CUBIC) on uint8 BGR (detect_precise, pose_detector.py:443) ----

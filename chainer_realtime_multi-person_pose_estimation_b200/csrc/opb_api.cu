@@ -34,6 +34,7 @@ using namespace opb;
 static_assert(sizeof(opb_person) == sizeof(PersonOut), "opb_person layout");
 static_assert(sizeof(opb_person) == 240, "opb_person size");
 static_assert(sizeof(opb_image_header) == sizeof(ImageHeader), "opb_image_header layout");
+static_assert(sizeof(opb_crop) == 24, "opb_crop size");
 
 namespace {
 
@@ -124,11 +125,13 @@ struct PostWs {           // post-process workspace for (N, map_h, map_w)
 
 struct KpWs {             // face / hand post-process workspace (grown on demand)
   size_t cap = 0;             // floats per buffer
-  int planes = 0;
-  float* up = nullptr;        // upsampled maps [planes][H][W]
+  int records = 0;            // capacity of res / h_res
+  int n_crops = 0;            // capacity of crops
+  float* up = nullptr;        // upsampled maps, ragged: crop i's [planes][h_i][w_i] at KpCrop::off
   float* tmp = nullptr;       // after the axis-0 pass
-  ChannelMax* res = nullptr;  // [planes]
+  ChannelMax* res = nullptr;  // [crops][planes]
   ChannelMax* h_res = nullptr;  // pinned
+  KpCrop* crops = nullptr;    // crop table of the current call
 };
 
 }  // namespace
@@ -1136,6 +1139,7 @@ void opb_destroy(opb_ctx* ctx) {
   if (ctx->ov_buf) cudaFree(ctx->ov_buf);
   if (ctx->kp_ws) {
     cudaFree(ctx->kp_ws->up); cudaFree(ctx->kp_ws->tmp); cudaFree(ctx->kp_ws->res); cudaFreeHost(ctx->kp_ws->h_res);
+    cudaFree(ctx->kp_ws->crops);
     delete ctx->kp_ws;
   }
   for (auto& sl : ctx->slots) {
@@ -2175,37 +2179,50 @@ int opb_stream_collect(opb_ctx* ctx, int slot, opb_image_header* headers_out, op
   return OPB_OK;
 }
 
-static int kp_workspace(opb_ctx* ctx, int planes, int H, int W, KpWs** out) {
+// Grows the face / hand workspace to at least `floats` per map buffer, `records` arg-max records and `n_crops` table
+// entries (keeping the larger of the old and the requested sizes).
+static int kp_workspace(opb_ctx* ctx, size_t floats, int records, int n_crops, KpWs** out) {
   if (!ctx->kp_ws) ctx->kp_ws = new KpWs();
   KpWs* ws = ctx->kp_ws;
-  const size_t need = static_cast<size_t>(planes) * H * W;
-  if (ws->cap < need || ws->planes < planes) {
+  if (ws->cap < floats || ws->records < records || ws->n_crops < n_crops) {
     OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ws->up); cudaFree(ws->tmp); cudaFree(ws->res); cudaFreeHost(ws->h_res);
-    ws->up = ws->tmp = nullptr; ws->res = nullptr; ws->h_res = nullptr; ws->cap = 0; ws->planes = 0;
-    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->up), need * 4));
-    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->tmp), need * 4));
-    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->res), sizeof(ChannelMax) * planes));
-    OPB_CUDA(ctx, cudaMallocHost(reinterpret_cast<void**>(&ws->h_res), sizeof(ChannelMax) * planes));
-    ws->cap = need; ws->planes = planes;
+    cudaFree(ws->up); cudaFree(ws->tmp); cudaFree(ws->res); cudaFreeHost(ws->h_res); cudaFree(ws->crops);
+    ws->up = ws->tmp = nullptr; ws->res = nullptr; ws->h_res = nullptr; ws->crops = nullptr;
+    const size_t cap = std::max(ws->cap, floats);
+    const int rec = std::max(ws->records, records), nc = std::max(ws->n_crops, n_crops);
+    ws->cap = 0; ws->records = 0; ws->n_crops = 0;
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->up), cap * 4));
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->tmp), cap * 4));
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->res), sizeof(ChannelMax) * rec));
+    OPB_CUDA(ctx, cudaMallocHost(reinterpret_cast<void**>(&ws->h_res), sizeof(ChannelMax) * rec));
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ws->crops), sizeof(KpCrop) * nc));
+    ws->cap = cap; ws->records = rec; ws->n_crops = nc;
   }
   *out = ws;
   return OPB_OK;
 }
 
-// smooth ws->up [planes][H][W] (both passes), per-plane maximum, records to the host
-static int kp_peaks(opb_ctx* ctx, KpWs* ws, int planes, int H, int W, int mirror, double thresh, double* out, int32_t* valid) {
-  dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, planes);
-  gauss_pass_kernel<0><<<grid, block, 0, ctx->stream>>>(ws->up, ws->tmp, H, W, ctx->taps);
-  gauss_pass_kernel<1><<<grid, block, 0, ctx->stream>>>(ws->tmp, ws->up, H, W, ctx->taps);
-  channel_argmax_kernel<<<planes, 256, 0, ctx->stream>>>(ws->up, H, W, mirror, ws->res);
-  ctx->launches += 3;
-  OPB_CUDA(ctx, cudaGetLastError());
-  OPB_CUDA(ctx, cudaMemcpyAsync(ws->h_res, ws->res, sizeof(ChannelMax) * planes, cudaMemcpyDeviceToHost, ctx->stream));
-  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+// Lays out the ragged workspace for `table` (h, w set): map offsets and tile numbers from host prefix sums.
+// Returns the number of 32x8 tiles and the floats the maps of `planes` channels need.
+static void kp_layout(std::vector<KpCrop>& table, int planes, long long* tiles, size_t* floats) {
+  size_t off = 0;
+  long long t = 0;
+  for (KpCrop& c : table) {
+    c.off = static_cast<long long>(off);
+    c.tile0 = static_cast<int>(std::min<long long>(t, INT32_MAX));   // callers reject tables with more than 2^30 tiles
+    off += static_cast<size_t>(planes) * c.h * c.w;
+    t += static_cast<long long>((c.w + 31) / 32) * ((c.h + 7) / 8);
+  }
+  *tiles = t;
+  *floats = off;
+}
+
+// One crop's arg-max records -> (x, y, conf) / valid, read the way compute_peaks_from_heatmaps reads them
+// (face_detector.py:55-67).  Shared by the single-crop and the batched entry points.
+static void kp_records_to_keypoints(const ChannelMax* res, int planes, int W, double thresh, double* out, int32_t* valid) {
   const float th = static_cast<float>(thresh);      // `max_value > thresh` with a float32 max_value compares in float32
   for (int c = 0; c < planes; ++c) {
-    const ChannelMax& r = ws->h_res[c];
+    const ChannelMax& r = res[c];
     valid[c] = r.value > th ? 1 : 0;
     // np.array(np.where(g == m)).flatten() = [y0..yk-1, x0..xk-1]; the reference reads [1] as x and [0] as y
     const int y0 = r.key0 / W, x0 = r.key0 - y0 * W;
@@ -2213,6 +2230,41 @@ static int kp_peaks(opb_ctx* ctx, KpWs* ws, int planes, int H, int W, int mirror
     out[c * 3 + 1] = static_cast<double>(y0);
     out[c * 3 + 2] = static_cast<double>(r.value);
   }
+}
+
+// Smooths the ragged maps in ws->up (both passes) and takes every (crop, plane) maximum; one copy of the records to
+// the host, one synchronisation, then the host conversion.  ws->crops must already hold `table`.
+static int kp_peaks(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, int planes, int tiles, double thresh,
+                    double* out, int32_t* valid) {
+  const int n = static_cast<int>(table.size());
+  dim3 block(32, 8), grid(tiles, planes);
+  gauss_pass_ragged_kernel<0><<<grid, block, 0, ctx->stream>>>(ws->up, ws->tmp, ws->crops, n, ctx->taps);
+  gauss_pass_ragged_kernel<1><<<grid, block, 0, ctx->stream>>>(ws->tmp, ws->up, ws->crops, n, ctx->taps);
+  channel_argmax_ragged_kernel<<<dim3(planes, n), 256, 0, ctx->stream>>>(ws->up, ws->crops, ws->res);
+  ctx->launches += 3;
+  OPB_CUDA(ctx, cudaGetLastError());
+  OPB_CUDA(ctx, cudaMemcpyAsync(ws->h_res, ws->res, sizeof(ChannelMax) * planes * n, cudaMemcpyDeviceToHost, ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < n; ++i)
+    kp_records_to_keypoints(ws->h_res + static_cast<size_t>(i) * planes, planes, table[i].w, thresh,
+                            out + static_cast<size_t>(i) * planes * 3, valid + static_cast<size_t>(i) * planes);
+  return OPB_OK;
+}
+
+// Workspace and device crop table for the single-crop entry points: one [planes][h][w] map set at offset 0.
+static int kp_single(opb_ctx* ctx, int planes, int h, int w, int mirror, std::vector<KpCrop>& table, int* tiles,
+                     KpWs** ws) {
+  KpCrop c{};
+  c.h = h; c.w = w; c.flip = mirror ? 1 : 0;
+  table.assign(1, c);
+  size_t floats = 0;
+  long long t = 0;
+  kp_layout(table, planes, &t, &floats);
+  if (t > (1 << 30)) OPB_FAIL(ctx, OPB_ERR_ARG, "maps too large");
+  *tiles = static_cast<int>(t);
+  int rc = kp_workspace(ctx, floats, planes, 1, ws);
+  if (rc) return rc;
+  OPB_CUDA(ctx, cudaMemcpyAsync((*ws)->crops, table.data(), sizeof(KpCrop), cudaMemcpyHostToDevice, ctx->stream));
   return OPB_OK;
 }
 
@@ -2221,10 +2273,12 @@ int opb_keypoints_from_heatmaps(opb_ctx* ctx, const float* heat, int heat_loc, i
   if (!ctx || !heat || !out || !valid || planes <= 0 || h <= 0 || w <= 0) return OPB_ERR_ARG;
   cudaSetDevice(ctx->device);
   KpWs* ws = nullptr;
-  int rc = kp_workspace(ctx, planes, h, w, &ws);
+  std::vector<KpCrop> table;
+  int tiles = 0;
+  int rc = kp_single(ctx, planes, h, w, mirror, table, &tiles, &ws);
   if (rc) return rc;
   if ((rc = copy_in(ctx, ws->up, heat, static_cast<size_t>(planes) * h * w * 4, heat_loc))) return rc;
-  return kp_peaks(ctx, ws, planes, h, w, mirror, thresh, out, valid);
+  return kp_peaks(ctx, ws, table, planes, tiles, thresh, out, valid);
 }
 
 int opb_keypoints_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int img_h, int img_w, int net_size, int mirror,
@@ -2248,11 +2302,87 @@ int opb_keypoints_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int img_
   if ((rc = run_chain(ctx, ch, true))) return rc;
   const int planes = ctx->kp_out - 1;              // the last channel is background (face_detector.py:59)
   KpWs* ws = nullptr;
-  if ((rc = kp_workspace(ctx, planes, img_h, img_w, &ws))) return rc;
+  std::vector<KpCrop> table;
+  int tiles = 0;
+  if ((rc = kp_single(ctx, planes, img_h, img_w, mirror, table, &tiles, &ws))) return rc;
   // F.resize_images(hs[-1], (crop_h, crop_w)) (face_detector.py:38)
   if ((rc = launch_upsample(ctx, ch->heat_lo, planes, net_size / 8, net_size / 8, ws->up, img_h, img_w))) return rc;
   if (maps_out && (rc = copy_out(ctx, maps_out, ws->up, static_cast<size_t>(planes) * img_h * img_w * 4, OPB_HOST))) return rc;
-  return kp_peaks(ctx, ws, planes, img_h, img_w, mirror, thresh, out, valid);
+  return kp_peaks(ctx, ws, table, planes, tiles, thresh, out, valid);
+}
+
+// Batch slots of the next forward chunk for `remaining` crops: full chunks of kKpMaxChunk, then the remainder rounded
+// up to a power of two, so that at most log2(kKpMaxChunk) + 1 chain shapes are ever built per net size.
+static const int kKpMaxChunk = 16;
+static int kp_chunk_slots(int remaining) {
+  if (remaining >= kKpMaxChunk) return kKpMaxChunk;
+  int p = 1;
+  while (p < remaining) p <<= 1;
+  return p;
+}
+
+int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int frame_h, int frame_w,
+                               const opb_crop* crops, int n, int net_size, double thresh, double* out, int32_t* valid) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (!ctx->kp_out) OPB_FAIL(ctx, OPB_ERR_STATE, "this context holds the pose net: load FaceNet / HandNet weights first");
+  if (n < 0 || n > 65535) OPB_FAIL(ctx, OPB_ERR_ARG, "crop count must be in [0, 65535]");
+  if (n == 0) return OPB_OK;
+  if (!frame || !crops || !out || !valid || frame_h <= 0 || frame_w <= 0) OPB_FAIL(ctx, OPB_ERR_ARG, "bad frame or output");
+  if (net_size <= 0 || net_size % 8) OPB_FAIL(ctx, OPB_ERR_ARG, "net_size must be a positive multiple of 8");
+  const int planes = ctx->kp_out - 1;              // the last channel is background (face_detector.py:59)
+  std::vector<KpCrop> table(n);
+  for (int i = 0; i < n; ++i) {
+    const opb_crop& b = crops[i];
+    const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
+    if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "crop " + std::to_string(i) + " has a non-positive (or huge) width or height");
+    KpCrop& c = table[i];
+    c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip ? 1 : 0;
+    // cv2.resize's inverse scales, as launch_resize_u8 forms them
+    c.sx = 1.0 / (static_cast<double>(net_size) / c.w);
+    c.sy = 1.0 / (static_cast<double>(net_size) / c.h);
+  }
+  long long t = 0;
+  size_t floats = 0;
+  kp_layout(table, planes, &t, &floats);
+  if (t > (1 << 30) || floats / planes > (1ull << 31)) OPB_FAIL(ctx, OPB_ERR_ARG, "crops too large for one call");
+  const int tiles = static_cast<int>(t);
+  cudaSetDevice(ctx->device);
+  int rc;
+  KpWs* ws = nullptr;
+  if ((rc = kp_workspace(ctx, floats, planes * n, n, &ws))) return rc;
+  const uint8_t* d_frame = frame;
+  if (frame_loc == OPB_HOST) {
+    const size_t in_b = static_cast<size_t>(frame_h) * frame_w * 3;
+    if ((rc = ensure_ingest(ctx, in_b + 512))) return rc;
+    if ((rc = copy_in(ctx, ctx->ingest_buf, frame, in_b, OPB_HOST))) return rc;
+    d_frame = ctx->ingest_buf;
+  }
+  OPB_CUDA(ctx, cudaMemcpyAsync(ws->crops, table.data(), sizeof(KpCrop) * n, cudaMemcpyHostToDevice, ctx->stream));
+  for (int first = 0; first < n;) {
+    const int slots = kp_chunk_slots(n - first), nc = std::min(slots, n - first);
+    Chain* ch = nullptr;
+    if ((rc = get_chain(ctx, slots, net_size, net_size, &ch))) return rc;
+    // crop_image + flip + cv2.resize(crop, (net, net)) straight from the frame (face_detector.py:31); padding slots zeroed
+    dim3 rgrid((net_size + 31) / 32, (net_size + 7) / 8, slots);
+    crop_resize_linear_u8_kernel<<<rgrid, dim3(32, 8), 0, ctx->stream>>>(d_frame, frame_h, frame_w, ws->crops + first, nc,
+                                                                         ch->img_u8, net_size);
+    ctx->launches++;
+    OPB_CUDA(ctx, cudaGetLastError());
+    ch->img_u8_src = nullptr;
+    if ((rc = run_chain(ctx, ch, true))) return rc;
+    // F.resize_images(hs[-1], (crop_h, crop_w)) of every crop of the chunk (face_detector.py:38)
+    const int h8 = net_size / 8, tile_end = first + nc < n ? table[first + nc].tile0 : tiles;
+    const int ppb = 19;
+    dim3 ugrid(tile_end - table[first].tile0, (planes + ppb - 1) / ppb);
+    upsample_bilinear_ac_ragged_kernel<<<ugrid, dim3(32, 8), 0, ctx->stream>>>(
+        ch->heat_lo, static_cast<size_t>(ctx->kp_out) * h8 * h8, planes, h8, h8, ws->crops + first, nc,
+        table[first].tile0, ws->up, ppb);
+    ctx->launches++;
+    OPB_CUDA(ctx, cudaGetLastError());
+    first += nc;
+  }
+  return kp_peaks(ctx, ws, table, planes, tiles, thresh, out, valid);
 }
 
 void* opb_device_buffer(opb_ctx* ctx, int which) {

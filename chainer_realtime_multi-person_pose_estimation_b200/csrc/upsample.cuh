@@ -6,8 +6,12 @@
 //       y += w4*x11 in float32 (no FMA contraction) -> bit-exact vs the oracle.
 //   resize_cubic_kernel : cv2.resize(..., INTER_CUBIC) for float32 maps (pose_detector.py
 //       :461-467): Keys cubic A=-0.75, half-pixel centres, replicate border, float32 taps.
+//   upsample_bilinear_ac_ragged_kernel : the same F.resize_images for face / hand crops of different sizes in one
+//       launch (face_detector.py:38), each crop's maps to its own h x w.
 #pragma once
 #include <cuda_runtime.h>
+
+#include "ingest.cuh"   // KpCrop
 
 namespace opb {
 
@@ -223,6 +227,32 @@ __device__ __forceinline__ float ac_sample(const float* __restrict__ plane, int 
   r = __fadd_rn(r, __fmul_rn(t.w3, __ldg(q + w)));
   r = __fadd_rn(r, __fmul_rn(t.w4, __ldg(q + w + 1)));
   return r;
+}
+
+// Ragged align-corners upsample: crop i of crops[0..n) reads planes [0, planes) of in + i * in_stride ([..][h][w] low-res
+// maps of one batch slot) and writes its own [planes][crops[i].h][crops[i].w] at out + crops[i].off.  One block = one
+// 32x8 tile of one crop for `planes_per_block` planes; grid (tiles of crops[0..n), ceil(planes / planes_per_block)).
+// `tile_base` = crops[0].tile0.  Same operations as upsample_bilinear_ac_kernel (ac_* helpers): identical bits.
+__global__ void __launch_bounds__(256)
+upsample_bilinear_ac_ragged_kernel(const float* __restrict__ in, size_t in_stride, int planes, int h, int w,
+                                   const KpCrop* __restrict__ crops, int n, int tile_base, float* __restrict__ out,
+                                   int planes_per_block) {
+  const int t = tile_base + static_cast<int>(blockIdx.x);
+  const int i = kp_find_crop(crops, n, t);
+  const KpCrop c = crops[i];
+  const int tiles_x = (c.w + 31) / 32, tl = t - c.tile0;
+  const int x = (tl % tiles_x) * 32 + threadIdx.x, y = (tl / tiles_x) * 8 + threadIdx.y;
+  if (x >= c.w || y >= c.h) return;
+  const AcTap tap = ac_tap(ac_axis_frac(x, w, c.w, ac_step(w, c.w)), ac_axis_frac(y, h, c.h, ac_step(h, c.h)), w);
+  const int p_begin = blockIdx.y * planes_per_block, p_end = min(planes, p_begin + planes_per_block);
+  const size_t in_plane = static_cast<size_t>(h) * w, out_plane = static_cast<size_t>(c.h) * c.w;
+  const float* src = in + i * in_stride + p_begin * in_plane;
+  float* dst = out + c.off + p_begin * out_plane + static_cast<size_t>(y) * c.w + x;
+  for (int p = p_begin; p < p_end; ++p) {
+    __stcs(dst, ac_sample(src, w, tap));
+    src += in_plane;
+    dst += out_plane;
+  }
 }
 
 // ---- cv2 INTER_CUBIC for float32 (A = -0.75), separable, replicate border ------------------

@@ -42,6 +42,14 @@ class FaceDetector(object):
         return self.engine.keypoints_detect(face_img, params["face_inference_img_size"],
                                             params['face_heatmap_peak_thresh'])
 
+    def detect_crops(self, img, bboxes):
+        """Every face of one frame in one device pass: `img` uint8 [H,W,3], `bboxes` (left, top, right, bottom) integer
+        boxes as PoseDetector.crop_face returns them.  Result i == self(PoseDetector.crop_image(img, bboxes[i])), keypoints
+        in crop coordinates.  ValueError (before anything runs on the device) for a malformed box or an empty crop."""
+        table = _native.crop_table(bboxes)
+        return self.engine.keypoints_detect_crops(img, table, params["face_inference_img_size"],
+                                                  params['face_heatmap_peak_thresh'])
+
     def create_gaussian_kernel(self, sigma=1, ksize=5):
         """The 2-D kernel of the reference's GPU branch (face_detector.py:44-52); kept for API compatibility --
         peak extraction here follows the CPU branch (scipy gaussian_filter) exactly."""

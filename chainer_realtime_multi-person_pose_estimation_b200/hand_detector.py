@@ -46,6 +46,18 @@ class HandDetector(object):
         return self.engine.keypoints_detect(hand_img, params["hand_inference_img_size"],
                                             params['hand_heatmap_peak_thresh'], mirror=left)
 
+    def detect_crops(self, img, bboxes, hand_types):
+        """Every hand of one frame in one device pass: `img` uint8 [H,W,3], `bboxes` (left, top, right, bottom) integer
+        boxes as PoseDetector.crop_hands returns them, `hand_types` one per box.  Result i ==
+        self(PoseDetector.crop_image(img, bboxes[i]), hand_type=hand_types[i]): only "left" mirrors (:29), anything
+        else is a right hand.  ValueError (before anything runs on the device) for a malformed box or an empty crop."""
+        bboxes, hand_types = list(bboxes), list(hand_types)
+        if len(hand_types) != len(bboxes):
+            raise ValueError("%d boxes but %d hand types" % (len(bboxes), len(hand_types)))
+        table = _native.crop_table(bboxes, [t == "left" for t in hand_types])
+        return self.engine.keypoints_detect_crops(img, table, params["hand_inference_img_size"],
+                                                  params['hand_heatmap_peak_thresh'])
+
     def create_gaussian_kernel(self, sigma=1, ksize=5):
         """The 2-D kernel of the reference's GPU branch (hand_detector.py:44-52); kept for API compatibility --
         peak extraction here follows the CPU branch (scipy gaussian_filter) exactly."""

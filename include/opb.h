@@ -255,6 +255,23 @@ int opb_keypoints_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int img_
 int opb_keypoints_from_heatmaps(opb_ctx* ctx, const float* heat, int heat_loc, int planes, int h, int w,
                                 int mirror, double thresh, double* out, int32_t* valid);
 
+/* -- all face (or hand) crops of one frame in one call: the result for crop i equals opb_keypoints_detect on
+ *    flip_i(PoseDetector.crop_image(frame, bbox_i)) with mirror = flip_i, bit for bit at equal conv tile shapes.
+ *    The canvas of a crop is (bottom-top) x (right-left); frame pixels outside it are read as 0.  The frame
+ *    [frame_h, frame_w, 3] uint8 BGR is uploaded once (or read in place with OPB_DEVICE); crops run through the net
+ *    in chunks of at most 16 (full chunks of 16, then the remainder rounded up to a power of two), and the upsample,
+ *    smoothing and arg-max of all crops are ragged launches.  One device-to-host copy and one synchronisation per call.
+ *    out [n][C-1][3] = (x, y, conf) in crop coordinates, valid [n][C-1].  OPB_ERR_ARG for a crop with a non-positive
+ *    width or height (nothing is launched); n == 0 returns at once.                                        */
+typedef struct opb_crop {
+  int32_t left, top, right, bottom;   /* crop_image bbox; zero fill outside the frame                          */
+  int32_t flip;                       /* 1: cv2.flip(crop, 1) before the net, positions reported unflipped     */
+  int32_t reserved;
+} opb_crop;
+int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int frame_h, int frame_w,
+                               const opb_crop* crops, int n, int net_size, double thresh,
+                               double* out /* [n][C-1][3] */, int32_t* valid /* [n][C-1] */);
+
 /* device pointers of the last opb_detect_batch outputs/intermediates (valid until the next
  * call with a different shape): 0 paf_lo, 1 heat_lo, 2 pafs (full-res), 3 heatmaps (full-res),
  * 4 headers, 5 persons, 6 peak table ([N,max_peaks] of {int32 type,x,y; float score})       */
