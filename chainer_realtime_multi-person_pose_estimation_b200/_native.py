@@ -33,7 +33,12 @@ PERSON_DTYPE = np.dtype([("score", "<f8"), ("count", "<f8"), ("peak_id", "<i4", 
 HEADER_DTYPE = np.dtype([("n_peaks", "<i4"), ("n_persons", "<i4"), ("status", "<i4"), ("n_connections", "<i4")])
 CROP_DTYPE = np.dtype([("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bottom", "<i4"), ("flip", "<i4"),
                        ("reserved", "<i4")])      # opb_crop
+PART_DTYPE = np.dtype([("kind", "<i4"), ("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bottom", "<i4"),
+                       ("first_point", "<i4")])   # opb_part
+PART_FACE, PART_HAND = 0, 1
+PART_POINTS = {PART_FACE: 70, PART_HAND: 21}
 assert PERSON_DTYPE.itemsize == 240 and HEADER_DTYPE.itemsize == 16 and CROP_DTYPE.itemsize == 24
+assert PART_DTYPE.itemsize == 24
 
 
 def crop_table(bboxes, flips=None):
@@ -98,6 +103,8 @@ _SIGNATURES = {
                                        C.c_int]),
     "opb_draw_last_result": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
                                        C.c_void_p, C.c_int]),
+    "opb_draw_whole_body": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                      C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "opb_stream_submit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_int]),
     "opb_stream_collect": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -375,6 +382,29 @@ class Engine(object):
         out = np.empty_like(a)
         self._check(self.lib.opb_draw_last_result(self.ctx, int(image_index), _ptr(a), OPB_HOST, h, w, float(sx), float(sy),
                                                   _ptr(out), OPB_HOST))
+        return out
+
+    def draw_whole_body(self, img, poses, parts):
+        """The whole-body picture of demo.py:28-57 on the device (opb_draw_whole_body): poses float [P,18,3] as for
+        draw_person_pose; parts (kind, bbox, keypoints) with kind PART_FACE / PART_HAND, bbox (left, top, right, bottom)
+        and keypoints the [x, y, conf] / None list of the detectors, in crop coordinates."""
+        a = np.ascontiguousarray(img, np.uint8)
+        h, w, _ = a.shape
+        ip = np.ascontiguousarray(np.asarray(poses).round().astype('i').reshape(-1, 18, 3), np.int32)
+        table = np.zeros(len(parts), PART_DTYPE)
+        rows = []
+        for i, (kind, bbox, kps) in enumerate(parts):
+            table[i] = (kind,) + tuple(int(v) for v in bbox) + (len(rows),)
+            rows.extend((int(k[0]), int(k[1]), 1) if k else (0, 0, 0) for k in kps)
+        pts = np.array(rows, np.int64).reshape(-1, 3)
+        lim = np.iinfo(np.int32)
+        if pts.size and (pts.min() < lim.min or pts.max() > lim.max):
+            raise ValueError("a keypoint coordinate does not fit int32")
+        pts = np.ascontiguousarray(pts, np.int32)
+        out = np.empty_like(a)
+        self._check(self.lib.opb_draw_whole_body(self.ctx, _ptr(a), OPB_HOST, h, w, _ptr(ip) if len(ip) else None, len(ip),
+                                                 _ptr(table) if len(table) else None, len(table),
+                                                 _ptr(pts) if len(pts) else None, len(pts), _ptr(out), OPB_HOST))
         return out
 
     def detect_image(self, img, in_h, in_w, map_h, map_w, img_len=None):

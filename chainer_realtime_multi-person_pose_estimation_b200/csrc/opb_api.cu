@@ -35,6 +35,7 @@ static_assert(sizeof(opb_person) == sizeof(PersonOut), "opb_person layout");
 static_assert(sizeof(opb_person) == 240, "opb_person size");
 static_assert(sizeof(opb_image_header) == sizeof(ImageHeader), "opb_image_header layout");
 static_assert(sizeof(opb_crop) == 24, "opb_crop size");
+static_assert(sizeof(opb_part) == 24, "opb_part size");
 
 namespace {
 
@@ -1808,7 +1809,37 @@ static OverlayTables overlay_tables(const opb_ctx* ctx) {
   }
   for (int j = 0; j < OV_JOINTS; ++j)
     for (int c = 0; c < 3; ++c) tb.joint_color[j][c] = kJoint[j][c];
+  // params['face_line_indices'] (entity.py:130-140): polylines over keypoint ranges, the eyes and lips closed
+  static const int kFaceChains[9][3] = {{0, 16, 0}, {17, 21, 0}, {22, 26, 0}, {27, 30, 0}, {31, 35, 0},
+                                        {36, 41, 1}, {42, 47, 1}, {48, 59, 1}, {60, 67, 1}};
+  int n = 0;
+  for (const auto& ch : kFaceChains) {
+    for (int k = ch[0]; k < ch[1]; ++k, ++n) { tb.face_line[n][0] = static_cast<uint8_t>(k); tb.face_line[n][1] = static_cast<uint8_t>(k + 1); }
+    if (ch[2]) { tb.face_line[n][0] = static_cast<uint8_t>(ch[1]); tb.face_line[n][1] = static_cast<uint8_t>(ch[0]); ++n; }
+  }
+  // params['fingers_indices'] (entity.py:145-151): wrist 0, then four joints per finger; finger_colors of
+  // hand_detector.py:93-99, the face colour of face_detector.py:86,95, the box colour of demo.py:40
+  static const uint8_t kFinger[OV_FINGERS][3] = {{0, 0, 255}, {0, 255, 255}, {0, 255, 0}, {255, 0, 0}, {255, 0, 255}};
+  for (int f = 0; f < OV_FINGERS; ++f) {
+    for (int s = 0; s < OV_FINGER_SEGS; ++s) {
+      tb.finger[f][s][0] = static_cast<uint8_t>(s == 0 ? 0 : 4 * f + s);
+      tb.finger[f][s][1] = static_cast<uint8_t>(4 * f + s + 1);
+    }
+    for (int c = 0; c < 3; ++c) tb.finger_color[f][c] = kFinger[f][c];
+  }
+  for (int c = 0; c < 3; ++c) {
+    tb.face_color[c] = c < 2 ? 255 : 0;
+    tb.rect_color[c] = 255;
+  }
   return tb;
+}
+
+static int ov_reserve(opb_ctx* ctx, size_t need) {
+  if (ctx->ov_bytes >= need) return OPB_OK;
+  if (ctx->ov_buf) { cudaStreamSynchronize(ctx->stream); cudaFree(ctx->ov_buf); ctx->ov_buf = nullptr; ctx->ov_bytes = 0; }
+  OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ctx->ov_buf), need));
+  ctx->ov_bytes = need;
+  return OPB_OK;
 }
 
 // poses: device int [n_poses][18][3] when from_records == nullptr; otherwise the records of one image are converted first
@@ -1818,17 +1849,13 @@ static int overlay_run(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int
   const size_t px = static_cast<size_t>(h) * w, img_b = (px * 3 + 255) & ~size_t(255);
   const size_t prio_b = (px * 4 + 255) & ~size_t(255), poses_b = (static_cast<size_t>(n_poses > 0 ? n_poses : 1) * OV_JOINTS * 3 * 4 + 255) & ~size_t(255);
   const size_t need = 2 * img_b + prio_b + poses_b + 256;
-  if (ctx->ov_bytes < need) {
-    if (ctx->ov_buf) { cudaStreamSynchronize(ctx->stream); cudaFree(ctx->ov_buf); ctx->ov_buf = nullptr; ctx->ov_bytes = 0; }
-    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ctx->ov_buf), need));
-    ctx->ov_bytes = need;
-  }
+  int rc;
+  if ((rc = ov_reserve(ctx, need))) return rc;
   uint8_t* d_in = ctx->ov_buf;
   uint8_t* d_out = ctx->ov_buf + img_b;
   unsigned int* d_prio = reinterpret_cast<unsigned int*>(ctx->ov_buf + 2 * img_b);
   int* d_poses = reinterpret_cast<int*>(ctx->ov_buf + 2 * img_b + prio_b);
   int* d_bad = reinterpret_cast<int*>(ctx->ov_buf + 2 * img_b + prio_b + poses_b);
-  int rc;
   const uint8_t* d_src = img;
   if (img_loc == OPB_HOST) {
     if ((rc = copy_in(ctx, d_in, img, px * 3, OPB_HOST))) return rc;
@@ -1849,10 +1876,12 @@ static int overlay_run(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int
       if ((rc = copy_in(ctx, d_poses, host_poses, static_cast<size_t>(n_poses) * OV_JOINTS * 3 * 4, OPB_HOST))) return rc;
     }
     const int n_prim = n_poses * (OV_LIMBS + OV_JOINTS);
-    overlay_raster_kernel<<<(n_prim + 63) / 64, 64, 0, ctx->stream>>>(d_poses, n_poses, tb, d_prio, h, w, d_bad);
+    overlay_raster_kernel<<<(n_prim + 63) / 64, 64, 0, ctx->stream>>>(d_poses, n_poses, tb, d_prio, h, w, d_bad, nullptr, 0,
+                                                                         nullptr);
     ctx->launches++;
   }
-  overlay_paint_kernel<<<static_cast<unsigned>((px + 255) / 256), 256, 0, ctx->stream>>>(d_src, d_prio, static_cast<int>(px), n_poses, tb, d_dst);
+  overlay_paint_kernel<<<static_cast<unsigned>((px + 255) / 256), 256, 0, ctx->stream>>>(d_src, d_prio, static_cast<int>(px), n_poses, tb, d_dst,
+                                                                                        nullptr, 0);
   ctx->launches++;
   OPB_CUDA(ctx, cudaGetLastError());
   int bad = 0;
@@ -1881,6 +1910,83 @@ int opb_draw_last_result(opb_ctx* ctx, int image_index, const uint8_t* img, int 
   if (hd.status != 0) OPB_FAIL(ctx, hd.status, "the image's result carries an error status");
   return overlay_run(ctx, img, img_loc, h, w, nullptr, hd.n_persons,
                      ws->persons + static_cast<size_t>(image_index) * ctx->prm.max_persons, sx, sy, out, out_loc);
+}
+
+// ---- the whole-body picture of demo.py:28-57 on the device (face_detector.py:79-97, hand_detector.py:89-117;
+// csrc/overlay.cuh): one upload of the frame and of the tables, one raster and one paint launch, one download
+int opb_draw_whole_body(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, const int32_t* poses, int n_poses,
+                        const opb_part* parts, int n_parts, const int32_t* points, int n_points, uint8_t* out, int out_loc) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (!img || !out || h <= 0 || w <= 0 || n_poses < 0 || n_parts < 0 || n_points < 0 || (n_poses > 0 && !poses) ||
+      (n_parts > 0 && !parts) || (n_points > 0 && !points))
+    OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: bad image, pose, part or point arguments");
+  const long long n_prim = static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) + static_cast<long long>(n_parts) * OV_PART_STRIDE;
+  if (n_prim > (1ll << 30)) OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: too many poses / parts");
+  // the raster kernel reads everything below without bounds checks: validate it all before anything is enqueued
+  for (long long k = 0; k < static_cast<long long>(n_poses) * OV_JOINTS; ++k) {
+    const int32_t* a = poses + 3 * k;
+    if (a[2] != 0 && (a[0] < 0 || a[0] >= w || a[1] < 0 || a[1] >= h))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a joint lies outside the image");
+  }
+  auto big = [](long long v) { return v < -(1ll << 20) || v > (1ll << 20); };   // keeps the rasterisers' ints in range
+  for (int p = 0; p < n_parts; ++p) {
+    const opb_part& pt = parts[p];
+    const int count = pt.kind == OPB_PART_FACE ? OV_FACE_POINTS : pt.kind == OPB_PART_HAND ? OV_HAND_POINTS : -1;
+    if (count < 0) OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: unknown part kind");
+    if (pt.first_point < 0 || static_cast<long long>(pt.first_point) + count > n_points)
+      OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a part's points run past the point table");
+    if (big(pt.left) || big(pt.top) || big(pt.right) || big(pt.bottom))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a box coordinate exceeds 2^20 in magnitude");
+    for (int k = 0; k < count; ++k) {
+      const int32_t* a = points + 3 * (static_cast<long long>(pt.first_point) + k);
+      if (a[2] != 0 && (big(a[0]) || big(a[1]) || big(static_cast<long long>(a[0]) + pt.left) ||
+                        big(static_cast<long long>(a[1]) + pt.top)))
+        OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a keypoint coordinate exceeds 2^20 in magnitude");
+    }
+  }
+  cudaSetDevice(ctx->device);
+  // scratch: [frame in | frame out | priority plane | tables: int poses | parts | points]
+  const size_t px = static_cast<size_t>(h) * w, img_b = (px * 3 + 255) & ~size_t(255), prio_b = (px * 4 + 255) & ~size_t(255);
+  const size_t poses_n = static_cast<size_t>(n_poses) * OV_JOINTS * 3, parts_n = static_cast<size_t>(n_parts) * 6;
+  const size_t tab_n = poses_n + parts_n + static_cast<size_t>(n_points) * 3;
+  static_assert(sizeof(opb_part) == 6 * sizeof(int32_t) && sizeof(OvPart) == sizeof(opb_part), "opb_part layout");
+  int rc;
+  if ((rc = ov_reserve(ctx, 2 * img_b + prio_b + tab_n * 4 + 256))) return rc;
+  uint8_t* d_in = ctx->ov_buf;
+  uint8_t* d_out = ctx->ov_buf + img_b;
+  unsigned int* d_prio = reinterpret_cast<unsigned int*>(ctx->ov_buf + 2 * img_b);
+  int* d_tab = reinterpret_cast<int*>(ctx->ov_buf + 2 * img_b + prio_b);
+  int* d_bad = d_tab + tab_n;                 // never raised: the joints were checked above
+  const uint8_t* d_src = img;
+  if (img_loc == OPB_HOST) {
+    if ((rc = copy_in(ctx, d_in, img, px * 3, OPB_HOST))) return rc;
+    d_src = d_in;
+  }
+  uint8_t* d_dst = (out_loc == OPB_HOST) ? d_out : out;
+  if (tab_n) {
+    std::vector<int32_t> tab(tab_n);
+    std::copy(poses, poses + poses_n, tab.begin());
+    if (parts_n) std::memcpy(tab.data() + poses_n, parts, parts_n * 4);
+    std::copy(points, points + static_cast<size_t>(n_points) * 3, tab.begin() + poses_n + parts_n);
+    if ((rc = copy_in(ctx, d_tab, tab.data(), tab_n * 4, OPB_HOST))) return rc;
+  }
+  const int* d_poses = d_tab;
+  const OvPart* d_parts = reinterpret_cast<const OvPart*>(d_tab + poses_n);
+  const int* d_points = d_tab + poses_n + parts_n;
+  OPB_CUDA(ctx, cudaMemsetAsync(d_prio, 0, px * 4, ctx->stream));
+  const OverlayTables tb = overlay_tables(ctx);
+  if (n_prim > 0) {
+    overlay_raster_kernel<<<static_cast<unsigned>((n_prim + 63) / 64), 64, 0, ctx->stream>>>(d_poses, n_poses, tb, d_prio, h, w, d_bad,
+                                                                                          d_parts, n_parts, d_points);
+    ctx->launches++;
+  }
+  overlay_paint_kernel<<<static_cast<unsigned>((px + 255) / 256), 256, 0, ctx->stream>>>(d_src, d_prio, static_cast<int>(px), n_poses, tb, d_dst,
+                                                                                        d_parts, 1);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  if (out_loc == OPB_HOST && (rc = copy_out(ctx, out, d_dst, px * 3, OPB_HOST))) return rc;
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return OPB_OK;
 }
 
 static int launch_resize_u8(opb_ctx* ctx, const uint8_t* d_src, int n, int h0, int w0, uint8_t* d_dst, int h, int w,

@@ -14,6 +14,19 @@
 // primitive -- exactly the pixel the sequential overwrite order leaves.  All joints are inside the image by
 // construction (they are scaled peak positions), which is the case OpenCV's own pre-clipping leaves untouched; the entry
 // point rejects joints outside the image.
+//
+// The whole-body picture of demo.py:28-57 extends the same scheme.  After the skeleton primitives come the face / hand
+// parts in the caller's order, each part owning OV_PART_STRIDE consecutive priorities:
+//   face (face_detector.py:79-97)   70 dots cv2.circle(radius 2, filled), then the 63 face_line_indices segments
+//                                   cv2.line(thickness 1), then the crop rectangle;
+//   hand (hand_detector.py:89-117)  per finger and segment: dot a, dot b (radius 3), the segment (thickness 1), all in
+//                                   the finger's colour; then the crop rectangle;
+//   rectangle                       cv2.rectangle(thickness 1): PolyLine of the four closed edges with thickness 1.
+// A 1-px line is ThickLine with thickness <= 1, LINE_8 and shift 0, i.e. drawing.cpp Line(): LineIterator(img, p0, p1,
+// 8, leftToRight = true) -- clipLine on the unscaled image size when an end point lies outside, then Bresenham.  Parts
+// may lie partly or wholly outside the frame.  The paint pass composes cv2.addWeighted(img, 0.6, skeleton, 0.4, 0):
+// a pixel whose top primitive is a part takes the part's colour, a skeleton pixel blend(img, skeleton colour), any
+// other pixel keeps img (blend(a, a) == a for every uint8 a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,11 +36,23 @@ namespace opb {
 constexpr int OV_SHIFT = 16;
 constexpr long long OV_ONE = 1ll << OV_SHIFT;
 constexpr int OV_LIMBS = 19, OV_JOINTS = 18;
+constexpr int OV_FACE_POINTS = 70, OV_FACE_LINES = 63, OV_HAND_POINTS = 21, OV_FINGERS = 5, OV_FINGER_SEGS = 4;
+constexpr int OV_HAND_PRIMS = OV_FINGERS * OV_FINGER_SEGS * 3;                 // dot a, dot b, segment
+constexpr int OV_PART_STRIDE = OV_FACE_POINTS + OV_FACE_LINES + 1;             // the larger part, rectangle included
+constexpr int OV_PART_FACE = 0, OV_PART_HAND = 1;
 
 struct OverlayTables {
   int limb_a[OV_LIMBS], limb_b[OV_LIMBS];      // params['limbs_point'] (entity.py:85-105)
   uint8_t limb_color[OV_LIMBS][3];             // pose_detector.py:524-529 (written to channels 0,1,2 as given)
   uint8_t joint_color[OV_JOINTS][3];           // :531-535
+  uint8_t face_line[OV_FACE_LINES][2];         // params['face_line_indices'] (entity.py:130-141)
+  uint8_t finger[OV_FINGERS][OV_FINGER_SEGS][2];  // params['fingers_indices'] (entity.py:145-151)
+  uint8_t finger_color[OV_FINGERS][3];         // hand_detector.py:93-99
+  uint8_t face_color[3], rect_color[3];        // face_detector.py:86,95; demo.py:40,50,57
+};
+
+struct OvPart {                                // == opb_part (include/opb.h)
+  int kind, left, top, right, bottom, first_point;
 };
 
 struct OvCanvas {
@@ -127,6 +152,51 @@ __device__ inline void ov_line2(const OvCanvas& cv, long long x1, long long y1, 
     }
   }
   (void)x_step;
+}
+
+// drawing.cpp Line(img, p1, p2, color, 8): LineIterator(img, p1, p2, 8, leftToRight = true), every pixel it visits.
+// Coordinates are bounded by the entry point (|v| <= 2^20), so the int arithmetic below cannot overflow.
+__device__ inline void ov_line1(const OvCanvas& cv, int x1, int y1, int x2, int y2) {
+  if (static_cast<unsigned>(x1) >= static_cast<unsigned>(cv.W) || static_cast<unsigned>(x2) >= static_cast<unsigned>(cv.W) ||
+      static_cast<unsigned>(y1) >= static_cast<unsigned>(cv.H) || static_cast<unsigned>(y2) >= static_cast<unsigned>(cv.H)) {
+    long long a1 = x1, b1 = y1, a2 = x2, b2 = y2;    // clipLine(Size, Point&, Point&) widens to Point2l
+    if (!ov_clip_line(cv.W, cv.H, a1, b1, a2, b2)) return;
+    x1 = static_cast<int>(a1); y1 = static_cast<int>(b1);
+    x2 = static_cast<int>(a2); y2 = static_cast<int>(b2);
+  }
+  int dx = x2 - x1, dy = y2 - y1, delta_y = 1;
+  if (dx < 0) {                                      // leftToRight: walk from the other end
+    dx = -dx;
+    dy = -dy;
+    x1 = x2;
+    y1 = y2;
+  }
+  if (dy < 0) {
+    dy = -dy;
+    delta_y = -1;
+  }
+  const bool vert = dy > dx;
+  if (vert) { const int t = dx; dx = dy; dy = t; }
+  // 8-connectivity: the major axis advances every step, the minor one when err < 0
+  int err = dx - (dy + dy);
+  const int plus_delta = dx + dx, minus_delta = -(dy + dy);
+  int x = x1, y = y1;
+  for (int i = 0; i <= dx; ++i) {
+    cv.put(x, y);
+    const int mask = err < 0 ? -1 : 0;
+    err += minus_delta + (plus_delta & mask);
+    if (vert) { y += delta_y; x += 1 & mask; }
+    else { x += 1; y += delta_y & mask; }
+  }
+}
+
+// drawing.cpp rectangle(img, pt1, pt2, color, 1): PolyLine of the closed quad (l,t) (r,t) (r,b) (l,b), starting with
+// the closing edge, each edge a 1-px Line()
+__device__ inline void ov_rect1(const OvCanvas& cv, int l, int t, int r, int b) {
+  ov_line1(cv, l, b, l, t);
+  ov_line1(cv, l, t, r, t);
+  ov_line1(cv, r, t, r, b);
+  ov_line1(cv, r, b, l, b);
 }
 
 // drawing.cpp FillConvexPoly(img, v, 4, color, LINE_8, XY_SHIFT)
@@ -257,12 +327,42 @@ __global__ void overlay_poses_from_records_kernel(const int* __restrict__ rec_x,
   poses[3 * i + 2] = has ? 2 : 0;
 }
 
-// one thread per potential primitive: [n_poses * 19 limbs | n_poses * 18 joints] in the reference's drawing order.
-// `bad` is raised when a drawn joint lies outside the image.
+// primitive j (< OV_PART_STRIDE) of one face / hand part; pts: the part's (x, y, present) rows in crop coordinates
+__device__ inline void ov_part_primitive(const OvCanvas& cv, const OverlayTables& tb, const OvPart& pt, const int* pts, int j) {
+  if (pt.kind == OV_PART_FACE) {
+    if (j < OV_FACE_POINTS) {
+      const int* a = pts + 3 * j;
+      if (a[2]) ov_circle_fill(cv, a[0] + pt.left, a[1] + pt.top, 2);
+    } else if (j < OV_FACE_POINTS + OV_FACE_LINES) {
+      const int* a = pts + 3 * tb.face_line[j - OV_FACE_POINTS][0];
+      const int* b = pts + 3 * tb.face_line[j - OV_FACE_POINTS][1];
+      if (a[2] && b[2]) ov_line1(cv, a[0] + pt.left, a[1] + pt.top, b[0] + pt.left, b[1] + pt.top);
+    } else {
+      ov_rect1(cv, pt.left, pt.top, pt.right, pt.bottom);
+    }
+  } else if (j < OV_HAND_PRIMS) {
+    const int f = j / (OV_FINGER_SEGS * 3), r = j - f * (OV_FINGER_SEGS * 3), s = r / 3, step = r - 3 * s;
+    const int* a = pts + 3 * tb.finger[f][s][0];
+    const int* b = pts + 3 * tb.finger[f][s][1];
+    if (step == 0) {
+      if (a[2]) ov_circle_fill(cv, a[0] + pt.left, a[1] + pt.top, 3);
+    } else if (step == 1) {
+      if (b[2]) ov_circle_fill(cv, b[0] + pt.left, b[1] + pt.top, 3);
+    } else if (a[2] && b[2]) {
+      ov_line1(cv, a[0] + pt.left, a[1] + pt.top, b[0] + pt.left, b[1] + pt.top);
+    }
+  } else if (j == OV_HAND_PRIMS) {
+    ov_rect1(cv, pt.left, pt.top, pt.right, pt.bottom);
+  }
+}
+
+// one thread per potential primitive: [n_poses * 19 limbs | n_poses * 18 joints | n_parts * OV_PART_STRIDE part
+// primitives] in the reference's drawing order.  `bad` is raised when a drawn joint lies outside the image.
 __global__ void overlay_raster_kernel(const int* __restrict__ poses, int n_poses, OverlayTables tb, unsigned int* __restrict__ prio,
-                                      int H, int W, int* __restrict__ bad) {
+                                      int H, int W, int* __restrict__ bad, const OvPart* __restrict__ parts, int n_parts,
+                                      const int* __restrict__ points) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_limb = n_poses * OV_LIMBS, n_all = n_limb + n_poses * OV_JOINTS;
+  const int n_limb = n_poses * OV_LIMBS, n_skel = n_limb + n_poses * OV_JOINTS, n_all = n_skel + n_parts * OV_PART_STRIDE;
   if (i >= n_all) return;
   OvCanvas cv{prio, H, W, static_cast<unsigned int>(i) + 1u};
   if (i < n_limb) {
@@ -273,27 +373,52 @@ __global__ void overlay_raster_kernel(const int* __restrict__ poses, int n_poses
     if (a[2] == 0 || b[2] == 0) return;
     if (a[0] < 0 || a[0] >= W || a[1] < 0 || a[1] >= H || b[0] < 0 || b[0] >= W || b[1] < 0 || b[1] >= H) { atomicOr(bad, 1); return; }
     ov_thick_line2(cv, a[0], a[1], b[0], b[1]);
-  } else {
+  } else if (i < n_skel) {
     const int k = i - n_limb;
     const int* a = poses + static_cast<size_t>(k) * 3;
     if (a[2] == 0) return;
     if (a[0] < 0 || a[0] >= W || a[1] < 0 || a[1] >= H) { atomicOr(bad, 1); return; }
     ov_circle_fill(cv, a[0], a[1], 3);
+  } else {
+    const int q = i - n_skel, p = q / OV_PART_STRIDE;
+    const OvPart pt = parts[p];
+    ov_part_primitive(cv, tb, pt, points + static_cast<size_t>(pt.first_point) * 3, q - p * OV_PART_STRIDE);
   }
 }
 
-// canvas = orig_img.copy(), then every covered pixel takes the colour of its last primitive
+// cv2.addWeighted(a, 0.6, b, 0.4, 0) on uint8: saturate_cast<uchar>(a*0.6f + (b*0.4f + 0.f)) in float32, rounded half
+// to even (the same bits with or without a fused multiply-add for every (a, b) pair)
+__device__ __forceinline__ uint8_t ov_blend(uint8_t a, uint8_t b) {
+  const float r = __fadd_rn(__fmul_rn(static_cast<float>(a), 0.6f), __fadd_rn(__fmul_rn(static_cast<float>(b), 0.4f), 0.f));
+  const int v = __float2int_rn(r);
+  return static_cast<uint8_t>(v < 0 ? 0 : (v > 255 ? 255 : v));
+}
+
+// canvas = orig_img.copy(), then every covered pixel takes the colour of its last primitive.  blend != 0 (whole-body
+// picture): skeleton pixels take blend(img, skeleton colour) instead; part pixels always take the part's colour.
 __global__ void __launch_bounds__(256)
 overlay_paint_kernel(const uint8_t* __restrict__ img, const unsigned int* __restrict__ prio, int n_pix, int n_poses,
-                     OverlayTables tb, uint8_t* __restrict__ out) {
+                     OverlayTables tb, uint8_t* __restrict__ out, const OvPart* __restrict__ parts, int blend) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pix) return;
   const unsigned int t = prio[i];
   uint8_t c0 = img[3 * static_cast<size_t>(i)], c1 = img[3 * static_cast<size_t>(i) + 1], c2 = img[3 * static_cast<size_t>(i) + 2];
   if (t) {
-    const int k = static_cast<int>(t) - 1, n_limb = n_poses * OV_LIMBS;
-    const uint8_t* col = (k < n_limb) ? tb.limb_color[k % OV_LIMBS] : tb.joint_color[(k - n_limb) % OV_JOINTS];
-    c0 = col[0]; c1 = col[1]; c2 = col[2];
+    const int k = static_cast<int>(t) - 1, n_limb = n_poses * OV_LIMBS, n_skel = n_limb + n_poses * OV_JOINTS;
+    if (k < n_skel) {
+      const uint8_t* col = (k < n_limb) ? tb.limb_color[k % OV_LIMBS] : tb.joint_color[(k - n_limb) % OV_JOINTS];
+      if (blend) {
+        c0 = ov_blend(c0, col[0]); c1 = ov_blend(c1, col[1]); c2 = ov_blend(c2, col[2]);
+      } else {
+        c0 = col[0]; c1 = col[1]; c2 = col[2];
+      }
+    } else {
+      const int q = k - n_skel, p = q / OV_PART_STRIDE, j = q - p * OV_PART_STRIDE;
+      const uint8_t* col;
+      if (parts[p].kind == OV_PART_FACE) col = j < OV_FACE_POINTS + OV_FACE_LINES ? tb.face_color : tb.rect_color;
+      else col = j < OV_HAND_PRIMS ? tb.finger_color[j / (OV_FINGER_SEGS * 3)] : tb.rect_color;
+      c0 = col[0]; c1 = col[1]; c2 = col[2];
+    }
   }
   out[3 * static_cast<size_t>(i)] = c0;
   out[3 * static_cast<size_t>(i) + 1] = c1;

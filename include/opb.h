@@ -205,6 +205,27 @@ int opb_draw_person_pose(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, i
  * (sx = orig_w / map_w, sy = orig_h / map_h; 1, 1 after the precise path).                                        */
 int opb_draw_last_result(opb_ctx* ctx, int image_index, const uint8_t* img, int img_loc, int h, int w, double sx,
                          double sy, uint8_t* out, int out_loc);
+/* -- the whole-body result picture of demo.py:28-57 in one call: out = cv2.addWeighted(img, 0.6,
+ *    draw_person_pose(img, poses), 0.4, 0), then for every part in order its keypoints -- draw_face_keypoints
+ *    (face_detector.py:79-97: 70 dots of radius 2, then the 63 face_line_indices segments of thickness 1) or
+ *    draw_hand_keypoints (hand_detector.py:89-117: per finger segment dot, dot, line, in the finger's colour) at
+ *    (left, top) -- and then cv2.rectangle((left, top), (right, bottom), (255, 255, 255), 1).  Pixel-identical to
+ *    those cv2 calls (csrc/overlay.cuh), parts and boxes partly or wholly outside the frame included.
+ *    poses: host int32 [n_poses,18,3] as for opb_draw_person_pose (every present joint inside the image).
+ *    points: host int32 [n_points,3] = (x, y, present) in crop coordinates; part i reads rows first_point ..
+ *    first_point + 69 (face) or + 20 (hand).  One upload of the frame (none with OPB_DEVICE) and one of the tables,
+ *    two launches, one download and one synchronisation.  OPB_ERR_ARG (nothing enqueued) for an unknown kind, a
+ *    negative count, points past n_points, a present joint outside the image, or a box or drawn keypoint coordinate of
+ *    magnitude above 2^20.                                                                                      */
+enum { OPB_PART_FACE = 0, OPB_PART_HAND = 1 };
+typedef struct opb_part {
+  int32_t kind;                       /* OPB_PART_FACE (70 points) or OPB_PART_HAND (21 points)                 */
+  int32_t left, top, right, bottom;   /* the crop box of crop_face / crop_hands                                 */
+  int32_t first_point;                /* row of the part's first keypoint in points                             */
+} opb_part;
+int opb_draw_whole_body(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, const int32_t* poses,
+                        int n_poses, const opb_part* parts, int n_parts, const int32_t* points, int n_points,
+                        uint8_t* out, int out_loc);
 
 /* -- streaming mode: the camera loop of camera_pose_demo.py:20-31, pipelined.  Two slots; submit()
  *    enqueues [pinned staging ->] H2D on a copy stream, the device resize (if orig != in), the whole

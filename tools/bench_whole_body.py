@@ -6,15 +6,21 @@ box of PoseDetector.crop_face and the hand boxes of PoseDetector.crop_hands are 
 ways with the seeded He weights of FaceNet and HandNet:
   (a) per crop: FaceDetector(crop_image(...)) once per face, HandDetector(...) once per hand, as demo.py does;
   (b) batched:  FaceDetector.detect_crops(frame, faces) once, HandDetector.detect_crops(frame, hands, types) once.
-Host wall clock around work that ends in a device synchronise (every call of both variants synchronises before it
-returns), after every shape has been warmed up; variants alternate, the median of --reps repetitions is reported.
-The CocoPoseNet body pass of the same frame is timed once per run for scale.
+The result picture of demo.py (the blended skeleton of the P poses, then per person the face, left hand and right hand
+keypoints of (b) with their boxes) is composed two ways as well:
+  (c) host:   whole_body.draw_whole_body(frame, poses, parts), i.e. the cv2 calls demo.py makes;
+  (d) device: the same with engine= (opb_draw_whole_body: one upload, two launches, one download).
+Host wall clock around work that ends in a device synchronise (every device call synchronises before it returns),
+after every shape has been warmed up; variants alternate, the median of --reps repetitions is reported.
+The CocoPoseNet body pass of the same frame is timed once per run for scale.  (c) runs on the host CPU, whose model
+the result records next to the GPU's.
 
     python tools/bench_whole_body.py [--people 1 4 8 16] [--reps 20] [--equal-tiles] [--out FILE]
 
 --equal-tiles sets OPB_SMALL_BATCH=0 before any context is built, so batch 1 and batch n use the same conv tile shapes.
-Prints one JSON line: GPU name, power limit and SM clocks read in the same run, per-P times, launch counts and whether
-(a) and (b) returned identical keypoints.  Needs an H100; there is no CPU path."""
+Prints one JSON line: GPU name, power limit and SM clocks read in the same run, the host CPU model, per-P times, launch
+counts, whether (a) and (b) returned identical keypoints and whether (c) and (d) drew identical images.  Needs an H100;
+there is no CPU path."""
 import argparse
 import json
 import os
@@ -40,6 +46,24 @@ def _gpu_info():
     return {"name": name, "power_limit_w": pl, "sm_clock_mhz": sm, "sm_clock_max_mhz": sm_max}
 
 
+def _cpu_model():
+    """the host CPU's model name (lscpu, else /proc/cpuinfo) and its logical CPU count: the host composition runs on it"""
+    import platform
+    name = None
+    try:
+        r = subprocess.run(["lscpu"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+        name = next((ln.split(":", 1)[1].strip() for ln in r.stdout.splitlines() if ln.startswith("Model name")), None)
+    except OSError:
+        pass
+    if not name:
+        try:
+            with open("/proc/cpuinfo") as f:
+                name = next((ln.split(":", 1)[1].strip() for ln in f if ln.startswith("model name")), None)
+        except OSError:
+            pass
+    return "%s (%s, %d logical CPUs)" % (name or "model not reported", platform.machine(), os.cpu_count() or 0)
+
+
 def _people(n):
     """[P,18,3] float poses (x, y, 1) of synthetic stick figures on the 640x480 frame"""
     import importlib
@@ -49,18 +73,21 @@ def _people(n):
 
 
 def _boxes(pose_det, frame, poses):
-    faces, hands = [], []
+    """face boxes, (hand box, side) pairs, and the demo's drawing order: ("face" | "hand", index into faces / hands)"""
+    faces, hands, order = [], [], []
     for pose in poses:
         pose = pose.copy()                     # crop_hands moves the hand joints in place (reference behaviour)
         unit = pose_det.get_unit_length(pose)
         img, bbox = pose_det.crop_face(frame, pose, unit)
         if img is not None and img.size:
+            order.append(("face", len(faces)))
             faces.append(bbox)
         hd = pose_det.crop_hands(frame, pose, unit)
         for side in ("left", "right"):
             if hd[side] is not None and hd[side]["img"].size:
+                order.append(("hand", len(hands)))
                 hands.append((hd[side]["bbox"], side))
-    return faces, hands
+    return faces, hands, order
 
 
 def main():
@@ -79,6 +106,7 @@ def main():
     pkg = importlib.import_module(PKG)
     syn, PD = pkg.synthetic, importlib.import_module(PKG + ".pose_detector")
     FD, HD = importlib.import_module(PKG + ".face_detector"), importlib.import_module(PKG + ".hand_detector")
+    WB = importlib.import_module(PKG + ".whole_body")
     models = {k: importlib.import_module(PKG + ".models." + k) for k in ("CocoPoseNet", "FaceNet", "HandNet")}
     nets = {}
     for k, m in models.items():
@@ -113,7 +141,8 @@ def main():
     gpu_before = _gpu_info()
     rows = []
     for p in a.people:
-        faces, hands = _boxes(pose_det, frame, _people(p))
+        poses = _people(p)
+        faces, hands, order = _boxes(pose_det, frame, poses)
         for _ in range(2):                     # every chain shape of both variants
             per_crop(faces, hands)
             batched(faces, hands)
@@ -121,19 +150,31 @@ def main():
         l0 = launches(); rb = batched(faces, hands); lb = launches() - l0
         ba, bb = bits(ra), bits(rb)
         differ = sum(x != y for u, v in zip(ba, bb) for x, y in zip(u, v))
-        ta, tb = [], []
+        parts = [("face", faces[i], rb[0][i]) if k == "face" else ("hand", hands[i][0], rb[1][i]) for k, i in order]
+        eng = pose_det.engine
+        host_img = WB.draw_whole_body(frame, poses, parts)
+        l0 = eng.launch_count(); dev_img = WB.draw_whole_body(frame, poses, parts, engine=eng); ld = eng.launch_count() - l0
+        ta, tb, tc, td = [], [], [], []
         for _ in range(a.reps):
             t0 = time.perf_counter(); per_crop(faces, hands); ta.append(time.perf_counter() - t0)
             t0 = time.perf_counter(); batched(faces, hands); tb.append(time.perf_counter() - t0)
+        for _ in range(a.reps):
+            t0 = time.perf_counter(); WB.draw_whole_body(frame, poses, parts); tc.append(time.perf_counter() - t0)
+            t0 = time.perf_counter(); WB.draw_whole_body(frame, poses, parts, engine=eng); td.append(time.perf_counter() - t0)
         rows.append({"people": p, "faces": len(faces), "hands": len(hands),
                      "per_crop_ms": round(float(np.median(ta)) * 1e3, 3), "batched_ms": round(float(np.median(tb)) * 1e3, 3),
                      "per_crop_ms_min": round(min(ta) * 1e3, 3), "batched_ms_min": round(min(tb) * 1e3, 3),
                      "speedup": round(float(np.median(ta) / np.median(tb)), 2),
                      "launches_per_crop": la, "launches_batched": lb,
-                     "identical": ba == bb, "keypoints_differing": int(differ), "keypoints_total": sum(len(u) for u in ba)})
+                     "identical": ba == bb, "keypoints_differing": int(differ), "keypoints_total": sum(len(u) for u in ba),
+                     "compose_host_ms": round(float(np.median(tc)) * 1e3, 3),
+                     "compose_device_ms": round(float(np.median(td)) * 1e3, 3),
+                     "compose_speedup": round(float(np.median(tc) / np.median(td)), 2),
+                     "launches_compose_device": ld, "images_identical": bool(np.array_equal(host_img, dev_img))})
     res = {"tool": "bench_whole_body", "frame": "640x480", "precision": "comp", "equal_tiles": bool(a.equal_tiles),
-           "reps": a.reps, "gpu": gpu_before, "gpu_after": _gpu_info(), "body_pass_ms": round(body_ms, 3), "rows": rows,
-           "identical": all(r["identical"] for r in rows)}
+           "reps": a.reps, "gpu": gpu_before, "gpu_after": _gpu_info(), "host_cpu": _cpu_model(),
+           "body_pass_ms": round(body_ms, 3), "rows": rows,
+           "identical": all(r["identical"] for r in rows), "images_identical": all(r["images_identical"] for r in rows)}
     line = json.dumps(res)
     print(line)
     if a.out:
