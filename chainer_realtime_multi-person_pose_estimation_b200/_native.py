@@ -134,6 +134,8 @@ _SIGNATURES = {
     "opb_time_stage": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_float)]),
     "opb_test_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "opb_test_conv_first": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                      C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 _lib = None
@@ -616,3 +618,19 @@ class Engine(object):
         self._check(self.lib.opb_test_conv(self.ctx, _ptr(x), n, h, w, cin, _ptr(W), _ptr(b), cout, ks,
                                            int(bool(relu)) | (2 if pool else 0), int(precision), _ptr(y)))
         return y
+
+    def test_conv_first(self, x, W, b, precision, u8_denom=255.0):
+        """conv1_1 alone: x uint8 [N,H,W,3] BGR or float32 [N,3,H,W] (preprocessed), W [64,3,3,3], b [64].
+        Returns the raw output tensor as uint8 [N,H,W,128] (fast) or [N,H,W,256] (parity, compensated)."""
+        is_u8 = np.asarray(x).dtype == np.uint8
+        x = np.ascontiguousarray(x, np.uint8 if is_u8 else np.float32)
+        W = np.ascontiguousarray(W, np.float32)
+        b = np.ascontiguousarray(b, np.float32)
+        if is_u8:
+            n, h, w, _ = x.shape
+        else:
+            n, _, h, w = x.shape
+        out = np.empty((n, h, w, 128 if int(precision) == PRECISION_FAST else 256), np.uint8)
+        self._check(self.lib.opb_test_conv_first(self.ctx, _ptr(x), int(is_u8), n, h, w, float(u8_denom), _ptr(W),
+                                                 _ptr(b), int(precision), _ptr(out)))
+        return out

@@ -336,6 +336,26 @@ int launch_conv(opb_ctx* ctx, const Op& op) {
   OPB_FAIL(ctx, OPB_ERR_UNSUPPORTED, "no conv kernel variant for ks " + std::to_string(op.ks));
 }
 
+template <int MODE>
+int launch_first_t(opb_ctx* ctx, const Chain* ch, const Op& op) {
+  auto kern = conv_first_kernel<MODE>;
+  constexpr int smem = conv_first_smem_bytes(MODE);
+  static bool attr_set[64] = {};
+  if (!attr_set[ctx->device & 63]) {
+    OPB_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set[ctx->device & 63] = true;
+  }
+  // persistent: two resident blocks per SM (register bound), each walking the tiles with a grid stride
+  const int tiles = op.N * ((op.H + CF_TH - 1) / CF_TH) * ((op.W + CF_TW - 1) / CF_TW);
+  const int grid = std::min(tiles, ctx->num_sms * 2);
+  kern<<<grid, CF_THREADS, smem, ctx->stream>>>(op.C == 1 ? (ch->img_u8_src ? ch->img_u8_src : ch->img_u8) : nullptr,
+                                                op.C == 1 ? nullptr : ch->img_f32, ctx->w_first, ctx->b_first,
+                                                reinterpret_cast<uint8_t*>(op.out), op.N, op.H, op.W, ctx->u8_denom);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  return OPB_OK;
+}
+
 int launch_op(opb_ctx* ctx, const Chain* ch, const Op& op) {
   if (op.kind == OP_CONV) return launch_conv(ctx, op);
   if (op.kind == OP_POOL) {
@@ -347,15 +367,14 @@ int launch_op(opb_ctx* ctx, const Chain* ch, const Op& op) {
     return OPB_OK;
   }
   // OP_FIRST
-  const int tiles = op.N * ((op.H + CF_TH - 1) / CF_TH) * ((op.W + CF_TW - 1) / CF_TW);
-  const int grid = std::min(tiles, ctx->num_sms * 8);
-  conv_first_kernel<<<grid, 256, 0, ctx->stream>>>(op.C == 1 ? (ch->img_u8_src ? ch->img_u8_src : ch->img_u8) : nullptr,
-                                                   op.C == 1 ? nullptr : ch->img_f32, ctx->w_first, ctx->b_first,
-                                                   op.out, op.N, op.H, op.W, op.cstride, op.lo_off, ctx->u8_denom,
-                                                   ctx->precision == OPB_PRECISION_COMP ? 1 : 0);
-  ctx->launches++;
-  OPB_CUDA(ctx, cudaGetLastError());
-  return OPB_OK;
+  const int mode = op.lo_off == 0 ? CF_FAST : ctx->precision == OPB_PRECISION_COMP ? CF_COMP : CF_PARITY;
+  if (op.cstride * 2 != conv_first_pix_bytes(mode) || (mode != CF_FAST && op.lo_off != 64))
+    OPB_FAIL(ctx, OPB_ERR_UNSUPPORTED, "conv1_1 output must be a dense 64-channel activation tensor");
+  switch (mode) {
+    case CF_FAST: return launch_first_t<CF_FAST>(ctx, ch, op);
+    case CF_PARITY: return launch_first_t<CF_PARITY>(ctx, ch, op);
+    default: return launch_first_t<CF_COMP>(ctx, ch, op);
+  }
 }
 
 // ------------------------------------------------------------------ weight packing
@@ -570,11 +589,9 @@ int build_chain(opb_ctx* ctx, Chain* ch, int N, int H, int W) {
   RC(alloc_act(ctx, ch, &SB, N, h8, w8, 256));
   RC(alloc_act(ctx, ch, &S512, N, h8, w8, 1024));
 
-  int first_rc = OPB_OK;
   auto first = [&]() {
     Op op; op.kind = OP_FIRST; op.tag = "conv1_1"; op.out = B0.p; op.N = N; op.H = H; op.W = W; op.C = 1;
     op.cstride = B0.Ctot; op.lo_off = split ? B0.C : 0;
-    first_rc = make_act_map(ctx, &op.tmA[0], B0, 0, 1);   // output tensor map of the tensor-core conv1_1 kernels (TMA store)
     ch->ops.push_back(op);
   };
   auto pool = [&](const char* tag, const Act& in, const Act& out) {
@@ -604,7 +621,6 @@ int build_chain(opb_ctx* ctx, Chain* ch, int N, int H, int W) {
   };
 
   first();
-  if (first_rc) return first_rc;
   // F.max_pooling_2d(2,2) (models/CocoPoseNet.py:138,141,146) is fused into the producing conv's epilogue
   if (fuse) { RC(conv1("conv1_2", B0, P1, 0, 64, 1)); } else { RC(conv1("conv1_2", B0, B1, 0, 64)); pool("pool1", B1, P1); }
   RC(conv1("conv2_1", P1, B2, 0, 128));
@@ -673,7 +689,6 @@ int build_chain_keypoint(opb_ctx* ctx, Chain* ch, int N, int H, int W) {
   {
     Op op; op.kind = OP_FIRST; op.tag = "conv1_1"; op.out = B0.p; op.N = N; op.H = H; op.W = W; op.C = 1;
     op.cstride = B0.Ctot; op.lo_off = split ? B0.C : 0;
-    RC(make_act_map(ctx, &op.tmA[0], B0, 0, 1));
     ch->ops.push_back(op);
   }
   auto conv = [&](const std::string& layer, const Act& in, const Act& out, int out_coff, int cout, int relu = 1,
@@ -2648,6 +2663,54 @@ int opb_test_conv(opb_ctx* ctx, const float* x, int n, int h, int w, int cin, co
   ctx->host_layers.erase("__test__");
   ctx->packed.erase("__test__");
   ctx->precision = saved_precision;
+  return rc;
+}
+
+int opb_test_conv_first(opb_ctx* ctx, const void* x, int x_is_u8, int n, int h, int w, float u8_denom, const float* W,
+                        const float* b, int precision_mode, uint8_t* out) {
+  if (!ctx || !x || !W || !b || !out || n <= 0 || h <= 0 || w <= 0) return OPB_ERR_ARG;
+  if (precision_mode != OPB_PRECISION_FAST && precision_mode != OPB_PRECISION_PARITY && precision_mode != OPB_PRECISION_COMP)
+    return OPB_ERR_ARG;
+  cudaSetDevice(ctx->device);
+  const size_t pixels = static_cast<size_t>(n) * h * w;
+  std::vector<float> wt(27 * 64);   // [27][64], k = (r*3+s)*3 + c, as load_weights packs conv1_1
+  for (int o = 0; o < 64; ++o)
+    for (int c = 0; c < 3; ++c)
+      for (int t = 0; t < 9; ++t) wt[(t * 3 + c) * 64 + o] = W[(static_cast<size_t>(o) * 3 + c) * 9 + t];
+  const int saved_precision = ctx->precision;
+  float* const saved_w = ctx->w_first;
+  float* const saved_b = ctx->b_first;
+  const float saved_denom = ctx->u8_denom;
+  Chain tmp;
+  Act y;
+  int rc = OPB_OK;
+  do {
+    ctx->precision = precision_mode;
+    if ((rc = dev_alloc(ctx, &ctx->w_first, wt.size(), tmp.allocs, false))) break;
+    if ((rc = dev_alloc(ctx, &ctx->b_first, 64, tmp.allocs, false))) break;
+    if (x_is_u8) { if ((rc = dev_alloc(ctx, &tmp.img_u8, pixels * 3, tmp.allocs, false))) break; }
+    else if ((rc = dev_alloc(ctx, &tmp.img_f32, pixels * 3, tmp.allocs, false))) break;
+    if ((rc = alloc_act(ctx, &tmp, &y, n, h, w, 64))) break;
+    ctx->u8_denom = u8_denom;
+    cudaError_t e = cudaMemcpyAsync(ctx->w_first, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->b_first, b, 64 * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess)
+      e = x_is_u8 ? cudaMemcpyAsync(tmp.img_u8, x, pixels * 3, cudaMemcpyHostToDevice, ctx->stream)
+                  : cudaMemcpyAsync(tmp.img_f32, x, pixels * 3 * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); rc = OPB_ERR_CUDA; break; }
+    Op op; op.kind = OP_FIRST; op.tag = "conv1_1"; op.out = y.p; op.N = n; op.H = h; op.W = w; op.C = x_is_u8 ? 1 : 0;
+    op.cstride = y.Ctot; op.lo_off = precision_mode == OPB_PRECISION_FAST ? 0 : y.C;
+    if ((rc = launch_op(ctx, &tmp, op))) break;
+    e = cudaMemcpyAsync(out, y.p, y.bytes(), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { ctx->err = std::string("test conv_first: ") + cudaGetErrorString(e); rc = OPB_ERR_CUDA; break; }
+  } while (0);
+  cudaStreamSynchronize(ctx->stream);
+  free_all(tmp.allocs);
+  ctx->precision = saved_precision;
+  ctx->w_first = saved_w;
+  ctx->b_first = saved_b;
+  ctx->u8_denom = saved_denom;
   return rc;
 }
 

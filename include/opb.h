@@ -346,6 +346,13 @@ int opb_time_stage(opb_ctx* ctx, const char* stage, int reps, float* ms);
  * then [N,H/2,W/2,Cout]).                                                                    */
 int opb_test_conv(opb_ctx* ctx, const float* x, int n, int h, int w, int cin, const float* W,
                   const float* b, int cout, int ksize, int relu, int precision_mode, float* y);
+/* conv1_1 alone (preprocess + 3x3 conv 3 -> 64 + ReLU), exactly as the chains run it.  x: uint8
+ * BGR [N,H,W,3] (x_is_u8 != 0, normalised as v / u8_denom - 0.5) or preprocessed float32
+ * [N,3,H,W]; W [64,3,3,3], b [64].  out receives the raw output tensor, N*H*W pixels of 128 B
+ * (fast: 64 fp16) or 256 B (parity: 64 fp16 hi | 64 fp16 lo; compensated: 64 fp16 hi |
+ * 64 B fp8(lo * 2^11) | 64 B fp8(v)).  The context's own conv1_1 weights are left untouched.  */
+int opb_test_conv_first(opb_ctx* ctx, const void* x, int x_is_u8, int n, int h, int w, float u8_denom,
+                        const float* W, const float* b, int precision_mode, uint8_t* out);
 
 #ifdef __cplusplus
 }
