@@ -136,6 +136,16 @@ _SIGNATURES = {
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "opb_test_conv_first": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "opb_cascade_load": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "opb_cascade_detect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
+                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
+    "opb_face_detect_frame": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int,
+                                        C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, C.c_void_p, C.c_int,
+                                        C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "opb_test_cascade_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
+                                           C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                           C.POINTER(C.c_int)]),
 }
 
 _lib = None
@@ -595,6 +605,82 @@ class Engine(object):
         heat = np.empty((19, h, w), np.float32)
         self._check(self.lib.opb_download_maps(self.ctx, _ptr(pafs), _ptr(heat), OPB_HOST))
         return pafs, heat
+
+    # -- Haar cascade (include/opb.h: opb_cascade_*) -------------------------------------------
+    def cascade_load(self, t):
+        """Load a cascade.HaarCascade into this context (one cascade per context; this replaces the previous one)."""
+        arrs = [np.ascontiguousarray(a, dt) for a, dt in
+                ((t.stage_ntrees, np.int32), (t.stage_threshold, np.float32), (t.stump_feature, np.int32),
+                 (t.stump_threshold, np.float32), (t.stump_left, np.float32), (t.stump_right, np.float32),
+                 (t.rects, np.int32), (t.weights, np.float32))]
+        ntrees, sthr, feat, thr, left, right, rects, weights = arrs
+        self._check(self.lib.opb_cascade_load(self.ctx, int(t.window[0]), int(t.window[1]), len(ntrees), _ptr(ntrees),
+                                              _ptr(sthr), len(feat), _ptr(feat), _ptr(thr), _ptr(left), _ptr(right),
+                                              len(rects), _ptr(rects), _ptr(weights)))
+        self.cascade_tables = t
+
+    @staticmethod
+    def _cascade_frame(img):
+        img = np.asarray(img)
+        if img.dtype != np.uint8 or not (img.ndim == 2 or (img.ndim == 3 and img.shape[2] in (1, 3))):
+            raise ValueError("image must be uint8 [H, W] gray or [H, W, 3] BGR, got %s %s" % (img.dtype, img.shape))
+        img = np.ascontiguousarray(img)
+        return img, img.shape[0], img.shape[1], (1 if img.ndim == 2 else img.shape[2])
+
+    @staticmethod
+    def _cascade_args(scale_factor, min_neighbors, min_size, max_size):
+        vals = [float(scale_factor), int(min_neighbors)] + [int(v) for v in tuple(min_size) + tuple(max_size)]
+        if len(vals) != 6:
+            raise ValueError("minSize and maxSize must be (w, h) pairs")
+        if not vals[0] > 1 or min(vals[1:]) < 0:
+            raise ValueError("scaleFactor must be > 1 and minNeighbors, minSize, maxSize must not be negative")
+        return vals
+
+    def cascade_detect(self, img, scale_factor, min_neighbors, min_size, max_size, cap=4096):
+        """detectMultiScale on the device (opb_cascade_detect): int32 [n, 4] rects sorted by (y, x, w, h)."""
+        img, h, w, ch = self._cascade_frame(img)
+        sf, mn, min_w, min_h, max_w, max_h = self._cascade_args(scale_factor, min_neighbors, min_size, max_size)
+        out = np.empty((cap, 4), np.int32)
+        n = C.c_int(0)
+        self._check(self.lib.opb_cascade_detect(self.ctx, _ptr(img), OPB_HOST, h, w, ch, sf, mn, min_w, min_h, max_w,
+                                                max_h, _ptr(out), cap, C.byref(n)))
+        return out[:n.value].copy()
+
+    def face_detect_frame(self, img, scale_factor, min_neighbors, min_size, max_size, crop_scale, net_size, thresh,
+                          cap=1024):
+        """camera_face_demo.py's frame on the device (opb_face_detect_frame): (rects int32 [n, 4], keypoint lists,
+        crop (left, top) pairs)."""
+        img, h, w, ch = self._cascade_frame(img)
+        if ch != 3:
+            raise ValueError("face_detect_frame needs a BGR [H, W, 3] frame")
+        sf, mn, min_w, min_h, max_w, max_h = self._cascade_args(scale_factor, min_neighbors, min_size, max_size)
+        planes = max(getattr(self, "kp_channels", 0) - 1, 0)   # 0 on a context without FaceNet: OPB_ERR_STATE
+        rects = np.empty((cap, 4), np.int32)
+        out = np.empty((cap, planes, 3), np.float64)
+        valid = np.empty((cap, planes), np.int32)
+        left_top = np.empty((cap, 2), np.int32)
+        n = C.c_int(0)
+        self._check(self.lib.opb_face_detect_frame(self.ctx, _ptr(img), OPB_HOST, h, w, sf, mn, min_w, min_h, max_w,
+                                                   max_h, float(crop_scale), int(net_size), float(thresh), _ptr(rects),
+                                                   cap, C.byref(n), _ptr(out), _ptr(valid), _ptr(left_top)))
+        k = n.value
+        return (rects[:k].copy(), [self._keypoint_list(o, v) for o, v in zip(out[:k], valid[:k])],
+                [(int(a), int(b)) for a, b in left_top[:k]])
+
+    def test_cascade_windows(self, img, scale_factor, min_size=(0, 0), max_size=(0, 0)):
+        """Test hook: (codes int32 [n], stage sums float64 [n]) of every window of every scale, before the skip rule."""
+        img, h, w, ch = self._cascade_frame(img)
+        sf, _, min_w, min_h, max_w, max_h = self._cascade_args(scale_factor, 0, min_size, max_size)
+        n = C.c_int(0)
+        rc = self.lib.opb_test_cascade_windows(self.ctx, _ptr(img), OPB_HOST, h, w, ch, sf, min_w, min_h, max_w, max_h,
+                                               None, None, 0, C.byref(n))
+        if rc not in (0, ERR_CAPACITY):
+            self._check(rc)
+        codes = np.empty(max(n.value, 1), np.int32)
+        sums = np.empty(max(n.value, 1), np.float64)
+        self._check(self.lib.opb_test_cascade_windows(self.ctx, _ptr(img), OPB_HOST, h, w, ch, sf, min_w, min_h, max_w,
+                                                      max_h, _ptr(codes), _ptr(sums), len(codes), C.byref(n)))
+        return codes[:n.value], sums[:n.value]
 
     # -- instrumentation ----------------------------------------------------------------------
     def device_buffer(self, which):

@@ -63,12 +63,15 @@ resize_linear_u8_kernel(const uint8_t* __restrict__ src, int h0, int w0, uint8_t
 // ---- face / hand crops straight from the frame (opb_keypoints_detect_crops) ----
 // One crop: the canvas of PoseDetector.crop_image (pose_detector.py:401-424) -- rows top..top+h-1, columns
 // left..left+w-1 of the frame, zero outside it -- optionally mirrored (cv2.flip(canvas, 1), hand_detector.py:29-30).
+// Only the canvas's top-left vh x vw pixels read the frame; the rest is zero.  crop_image canvases have vh = h,
+// vw = w; the padded squares of camera_face_demo.py's crop_face have edge x edge canvases over a smaller extent.
 // The same descriptor drives the ragged post-process kernels of keypoints.cuh / upsample.cuh.
 struct KpCrop {
   long long off;        // first float of the crop's maps [planes][h][w] in the ragged workspace
   int top, left, h, w;  // canvas origin in the frame and canvas size (= size of the crop's maps)
   int flip;             // canvas mirrored before the net; peak positions reported in the unmirrored canvas
   int tile0;            // first 32x8 tile of the crop in the ragged tile enumeration
+  int vh, vw;           // valid extent of the canvas (unmirrored): pixels with y >= vh or x >= vw are zero
   double sx, sy;        // cv2.resize scales canvas -> net: 1 / (net / w), 1 / (net / h)
 };
 
@@ -84,10 +87,11 @@ __device__ __forceinline__ int kp_find_crop(const KpCrop* __restrict__ crops, in
 
 struct CropCanvasU8 {       // crop_image(frame, bbox) (+ flip) read in place
   const uint8_t* frame;
-  int fh, fw, top, left, w, flip;
+  int fh, fw, top, left, w, flip, vh, vw;
   __device__ __forceinline__ int operator()(int y, int x, int c) const {
-    const int fy = top + y, fx = left + (flip ? w - 1 - x : x);
-    return (fy >= 0 && fy < fh && fx >= 0 && fx < fw) ? frame[(static_cast<size_t>(fy) * fw + fx) * 3 + c] : 0;
+    const int cx = flip ? w - 1 - x : x, fy = top + y, fx = left + cx;
+    return (y < vh && cx < vw && fy >= 0 && fy < fh && fx >= 0 && fx < fw)
+               ? frame[(static_cast<size_t>(fy) * fw + fx) * 3 + c] : 0;
   }
 };
 
@@ -101,7 +105,7 @@ crop_resize_linear_u8_kernel(const uint8_t* __restrict__ frame, int fh, int fw, 
   uint8_t* o = dst + ((static_cast<size_t>(n) * net + y) * net + x) * 3;
   if (n >= n_real) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
   const KpCrop k = crops[n];
-  const CropCanvasU8 s{frame, fh, fw, k.top, k.left, k.w, k.flip};
+  const CropCanvasU8 s{frame, fh, fw, k.top, k.left, k.w, k.flip, k.vh, k.vw};
   cv_linear_pixel(s, k.h, k.w, x, y, k.sx, k.sy, o);
 }
 

@@ -13,11 +13,13 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <queue>
 #include <vector>
 
 #include "../../include/opb.h"
+#include "cascade.cuh"
 #include "conv_first.cuh"
 #include "ingest.cuh"
 #include "overlay.cuh"
@@ -137,6 +139,8 @@ struct KpWs {             // face / hand post-process workspace (grown on demand
 
 }  // namespace
 
+struct CascadeState;
+
 struct opb_ctx {
   int device = 0;
   int num_sms = 132;
@@ -152,6 +156,7 @@ struct opb_ctx {
   int kp_out = 0;            // 0: CocoPoseNet; 71 / 22: FaceNet / HandNet (channels of the final 1x1, incl. background)
   float u8_denom = 255.f;    // uint8 normalisation: /255 (pose_detector.py:429) or /256 (face_detector.py:32)
   KpWs* kp_ws = nullptr;
+  CascadeState* cascade = nullptr;   // opb_cascade_load
   std::map<std::string, HostLayer> host_layers;
   std::map<std::string, PackedW> packed;
   float* w_first = nullptr;  // conv1_1 [27][64] fp32
@@ -1158,6 +1163,7 @@ void opb_destroy(opb_ctx* ctx) {
     cudaFree(ctx->kp_ws->crops);
     delete ctx->kp_ws;
   }
+  delete ctx->cascade;
   for (auto& sl : ctx->slots) {
     if (sl.d_frames) cudaFree(sl.d_frames);
     if (sl.h_frames) cudaFreeHost(sl.h_frames);
@@ -2442,23 +2448,14 @@ static int kp_chunk_slots(int remaining) {
   return p;
 }
 
-int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int frame_h, int frame_w,
-                               const opb_crop* crops, int n, int net_size, double thresh, double* out, int32_t* valid) {
-  if (!ctx) return OPB_ERR_ARG;
-  if (!ctx->kp_out) OPB_FAIL(ctx, OPB_ERR_STATE, "this context holds the pose net: load FaceNet / HandNet weights first");
-  if (n < 0 || n > 65535) OPB_FAIL(ctx, OPB_ERR_ARG, "crop count must be in [0, 65535]");
-  if (n == 0) return OPB_OK;
-  if (!frame || !crops || !out || !valid || frame_h <= 0 || frame_w <= 0) OPB_FAIL(ctx, OPB_ERR_ARG, "bad frame or output");
-  if (net_size <= 0 || net_size % 8) OPB_FAIL(ctx, OPB_ERR_ARG, "net_size must be a positive multiple of 8");
+// Crops of `table` (top, left, h, w, flip, vh, vw set) of a frame already on the device, through FaceNet / HandNet in
+// chunks of kp_chunk_slots: one crop-table upload, then per chunk a crop + resize launch, the chain and a ragged
+// upsample; then kp_peaks (one download, one synchronisation).  Keypoints of crop i in crop i's canvas coordinates.
+static int kp_detect_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, int frame_w, std::vector<KpCrop>& table,
+                           int net_size, double thresh, double* out, int32_t* valid) {
+  const int n = static_cast<int>(table.size());
   const int planes = ctx->kp_out - 1;              // the last channel is background (face_detector.py:59)
-  std::vector<KpCrop> table(n);
-  for (int i = 0; i < n; ++i) {
-    const opb_crop& b = crops[i];
-    const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
-    if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20))
-      OPB_FAIL(ctx, OPB_ERR_ARG, "crop " + std::to_string(i) + " has a non-positive (or huge) width or height");
-    KpCrop& c = table[i];
-    c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip ? 1 : 0;
+  for (KpCrop& c : table) {
     // cv2.resize's inverse scales, as launch_resize_u8 forms them
     c.sx = 1.0 / (static_cast<double>(net_size) / c.w);
     c.sy = 1.0 / (static_cast<double>(net_size) / c.h);
@@ -2468,17 +2465,9 @@ int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc
   kp_layout(table, planes, &t, &floats);
   if (t > (1 << 30) || floats / planes > (1ull << 31)) OPB_FAIL(ctx, OPB_ERR_ARG, "crops too large for one call");
   const int tiles = static_cast<int>(t);
-  cudaSetDevice(ctx->device);
   int rc;
   KpWs* ws = nullptr;
   if ((rc = kp_workspace(ctx, floats, planes * n, n, &ws))) return rc;
-  const uint8_t* d_frame = frame;
-  if (frame_loc == OPB_HOST) {
-    const size_t in_b = static_cast<size_t>(frame_h) * frame_w * 3;
-    if ((rc = ensure_ingest(ctx, in_b + 512))) return rc;
-    if ((rc = copy_in(ctx, ctx->ingest_buf, frame, in_b, OPB_HOST))) return rc;
-    d_frame = ctx->ingest_buf;
-  }
   OPB_CUDA(ctx, cudaMemcpyAsync(ws->crops, table.data(), sizeof(KpCrop) * n, cudaMemcpyHostToDevice, ctx->stream));
   for (int first = 0; first < n;) {
     const int slots = kp_chunk_slots(n - first), nc = std::min(slots, n - first);
@@ -2504,6 +2493,483 @@ int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc
     first += nc;
   }
   return kp_peaks(ctx, ws, table, planes, tiles, thresh, out, valid);
+}
+
+int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int frame_h, int frame_w,
+                               const opb_crop* crops, int n, int net_size, double thresh, double* out, int32_t* valid) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (!ctx->kp_out) OPB_FAIL(ctx, OPB_ERR_STATE, "this context holds the pose net: load FaceNet / HandNet weights first");
+  if (n < 0 || n > 65535) OPB_FAIL(ctx, OPB_ERR_ARG, "crop count must be in [0, 65535]");
+  if (n == 0) return OPB_OK;
+  if (!frame || !crops || !out || !valid || frame_h <= 0 || frame_w <= 0) OPB_FAIL(ctx, OPB_ERR_ARG, "bad frame or output");
+  if (net_size <= 0 || net_size % 8) OPB_FAIL(ctx, OPB_ERR_ARG, "net_size must be a positive multiple of 8");
+  std::vector<KpCrop> table(n);
+  for (int i = 0; i < n; ++i) {
+    const opb_crop& b = crops[i];
+    const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
+    if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "crop " + std::to_string(i) + " has a non-positive (or huge) width or height");
+    KpCrop& c = table[i];
+    c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip ? 1 : 0;
+    c.vh = c.h; c.vw = c.w;
+  }
+  cudaSetDevice(ctx->device);
+  int rc;
+  const uint8_t* d_frame = frame;
+  if (frame_loc == OPB_HOST) {
+    const size_t in_b = static_cast<size_t>(frame_h) * frame_w * 3;
+    if ((rc = ensure_ingest(ctx, in_b + 512))) return rc;
+    if ((rc = copy_in(ctx, ctx->ingest_buf, frame, in_b, OPB_HOST))) return rc;
+    d_frame = ctx->ingest_buf;
+  }
+  return kp_detect_table(ctx, d_frame, frame_h, frame_w, table, net_size, thresh, out, valid);
+}
+
+// ---------------------------------------------------------------- Haar cascade (csrc/cascade.cuh)
+namespace {
+
+const float kCascadeThresholdEps = 1e-5f;   // OpenCV's THRESHOLD_EPS, subtracted from stage thresholds at load
+const int kCascadeMaxRaw = 8192;            // raw candidates per frame (before grouping)
+
+int cv_round(double v) { return static_cast<int>(std::nearbyint(v)); }   // cvRound: half to even
+
+}  // namespace
+
+struct CascadeState {
+  int win_w = 0, win_h = 0;
+  std::vector<CascadeStage> stages;
+  std::vector<int> feat;                        // per stump
+  std::vector<float> sthr, sleft, sright;
+  std::vector<int> rects;                       // [F][3][4]
+  std::vector<float> weights;                   // [F][3]
+  CascadeStage* d_stages = nullptr;
+  CascadeStump* d_stumps = nullptr;
+  int stump_pitch = -1;                         // pitch the stump offsets were built for
+  // plan of the last (h, w, scale_factor, min, max)
+  struct Key { int h, w, min_w, min_h, max_w, max_h; double sf; } key{-1, -1, 0, 0, 0, 0, 0.0};
+  std::vector<CascadeLayer> layers;
+  int pitch = 0, rows = 0, n_windows = 0, max_h = 0, max_w = 0, max_ny = 0;
+  CascadeLayer* d_layers = nullptr;
+  CascadeAxis* d_axes = nullptr;
+  uint8_t* d_img = nullptr;
+  uint32_t *d_sum = nullptr, *d_sq = nullptr;
+  int* d_codes = nullptr;
+  double* d_sums = nullptr; size_t sums_cap = 0;
+  std::vector<void*> plan_allocs;
+  uint8_t* d_frame = nullptr; size_t frame_cap = 0;
+  int* d_cand = nullptr;
+  int* h_cand = nullptr;                        // pinned [1 + 3 * kCascadeMaxRaw]
+  void release_plan() { free_all(plan_allocs); d_layers = nullptr; d_axes = nullptr; d_img = nullptr; d_sum = d_sq = nullptr; d_codes = nullptr; key.h = -1; }
+  ~CascadeState() {
+    release_plan();
+    cudaFree(d_stages); cudaFree(d_stumps); cudaFree(d_sums); cudaFree(d_frame); cudaFree(d_cand); cudaFreeHost(h_cand);
+  }
+};
+
+namespace {
+
+// The float32 scale list of detectMultiScaleNoGrouping: factor *= scale_factor in double while cvRound(win * factor)
+// fits the frame and the maximum size; factors whose window is below the minimum size are skipped.
+std::vector<float> cascade_scales(const CascadeState* cs, int h, int w, double sf, int min_w, int min_h, int max_w,
+                                  int max_h) {
+  if (max_w == 0 || max_h == 0) { max_w = w; max_h = h; }
+  std::vector<float> out;
+  for (double factor = 1.0;; factor *= sf) {
+    const int ww = cv_round(cs->win_w * factor), wh = cv_round(cs->win_h * factor);
+    if (ww > max_w || wh > max_h || ww > w || wh > h) break;
+    if (ww < min_w || wh < min_h) continue;
+    out.push_back(static_cast<float>(factor));
+  }
+  return out;
+}
+
+void cascade_axis(int dst_n, int src_n, std::vector<CascadeAxis>& out) {
+  const double scale = 1.0 / (static_cast<double>(dst_n) / src_n);
+  for (int d = 0; d < dst_n; ++d) {
+    const double f = (d + 0.5) * scale - 0.5;
+    const double s = std::floor(f);
+    const int c1 = cv_round((f - s) * 256);
+    const int si = static_cast<int>(s);
+    out.push_back(CascadeAxis{std::min(std::max(si, 0), src_n - 1), std::min(std::max(si + 1, 0), src_n - 1), c1, 0});
+  }
+}
+
+// Layers, interpolation records and buffers for one (h, w, scale_factor, min, max); reused while the key holds.
+int cascade_plan(opb_ctx* ctx, CascadeState* cs, int h, int w, double sf, int min_w, int min_h, int max_w, int max_h) {
+  CascadeState::Key k{h, w, min_w, min_h, max_w, max_h, sf};
+  if (cs->key.h == k.h && cs->key.w == k.w && cs->key.min_w == k.min_w && cs->key.min_h == k.min_h &&
+      cs->key.max_w == k.max_w && cs->key.max_h == k.max_h && cs->key.sf == k.sf)
+    return OPB_OK;
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  cs->release_plan();
+  const std::vector<float> sc = cascade_scales(cs, h, w, sf, min_w, min_h, max_w, max_h);
+  cs->layers.clear();
+  std::vector<CascadeAxis> axes;
+  int row = 0, win = 0;
+  cs->max_h = cs->max_w = cs->max_ny = 0;
+  for (float s : sc) {
+    CascadeLayer L{};
+    L.scale = s;
+    L.w = cv_round(static_cast<float>(w) / s);
+    L.h = cv_round(static_cast<float>(h) / s);
+    L.ystep = s >= 2.f ? 1 : 2;
+    const int ww = L.w + 1 - cs->win_w, wh = L.h + 1 - cs->win_h;
+    L.nx = ww > 0 ? (ww + L.ystep - 1) / L.ystep : 0;
+    L.ny = wh > 0 ? (wh + L.ystep - 1) / L.ystep : 0;
+    if (L.nx == 0) L.ny = 0;
+    L.row0 = row;
+    L.win0 = win;
+    L.xtab = static_cast<int>(axes.size());
+    cascade_axis(L.w, w, axes);
+    L.ytab = static_cast<int>(axes.size());
+    cascade_axis(L.h, h, axes);
+    row += L.h + 1;
+    if (static_cast<long long>(win) + static_cast<long long>(L.nx) * L.ny > (1ll << 30))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "too many cascade windows for one frame");
+    win += L.nx * L.ny;
+    cs->max_h = std::max(cs->max_h, L.h);
+    cs->max_w = std::max(cs->max_w, L.w);
+    cs->max_ny = std::max(cs->max_ny, L.ny);
+    cs->layers.push_back(L);
+  }
+  cs->pitch = cs->max_w + 1;
+  cs->rows = row;
+  cs->n_windows = win;
+  if (cs->layers.empty()) { cs->key = k; return OPB_OK; }
+  if (cs->layers.size() > 65535) OPB_FAIL(ctx, OPB_ERR_ARG, "too many cascade scales");
+  const size_t cells = static_cast<size_t>(cs->pitch) * cs->rows;
+  int rc;
+  if ((rc = dev_alloc(ctx, &cs->d_layers, cs->layers.size(), cs->plan_allocs, false))) return rc;
+  if ((rc = dev_alloc(ctx, &cs->d_axes, axes.size(), cs->plan_allocs, false))) return rc;
+  if ((rc = dev_alloc(ctx, &cs->d_img, cells, cs->plan_allocs, false))) return rc;
+  if ((rc = dev_alloc(ctx, &cs->d_sum, cells, cs->plan_allocs, false))) return rc;
+  if ((rc = dev_alloc(ctx, &cs->d_sq, cells, cs->plan_allocs, false))) return rc;
+  if ((rc = dev_alloc(ctx, &cs->d_codes, std::max(win, 1), cs->plan_allocs, false))) return rc;
+  OPB_CUDA(ctx, cudaMemcpyAsync(cs->d_layers, cs->layers.data(), sizeof(CascadeLayer) * cs->layers.size(),
+                                cudaMemcpyHostToDevice, ctx->stream));
+  OPB_CUDA(ctx, cudaMemcpyAsync(cs->d_axes, axes.data(), sizeof(CascadeAxis) * axes.size(), cudaMemcpyHostToDevice,
+                                ctx->stream));
+  if (cs->stump_pitch != cs->pitch) {   // rect corners as offsets in this pitch
+    const int P = cs->pitch, T = static_cast<int>(cs->feat.size());
+    std::vector<CascadeStump> st(T);
+    for (int t = 0; t < T; ++t) {
+      CascadeStump& u = st[t];
+      for (int r = 0; r < 3; ++r) {
+        const int* q = &cs->rects[(static_cast<size_t>(cs->feat[t]) * 3 + r) * 4];
+        u.ofs[r][0] = q[1] * P + q[0];
+        u.ofs[r][1] = q[1] * P + q[0] + q[2];
+        u.ofs[r][2] = (q[1] + q[3]) * P + q[0];
+        u.ofs[r][3] = (q[1] + q[3]) * P + q[0] + q[2];
+        u.w[r] = cs->weights[static_cast<size_t>(cs->feat[t]) * 3 + r];
+      }
+      u.thr = cs->sthr[t]; u.left = cs->sleft[t]; u.right = cs->sright[t];
+    }
+    OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(cs->d_stumps);
+    cs->d_stumps = nullptr;
+    cs->stump_pitch = -1;
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&cs->d_stumps), sizeof(CascadeStump) * std::max(T, 1)));
+    OPB_CUDA(ctx, cudaMemcpyAsync(cs->d_stumps, st.data(), sizeof(CascadeStump) * T, cudaMemcpyHostToDevice, ctx->stream));
+    cs->stump_pitch = P;
+  }
+  cs->key = k;
+  return OPB_OK;
+}
+
+int cascade_check(opb_ctx* ctx, const uint8_t* img, int h, int w, int channels, double sf, int min_w, int min_h,
+                  int max_w, int max_h) {
+  if (!ctx->cascade) OPB_FAIL(ctx, OPB_ERR_STATE, "no cascade loaded: call opb_cascade_load first");
+  if (!img || h <= 0 || w <= 0) OPB_FAIL(ctx, OPB_ERR_ARG, "bad frame");
+  if (channels != 1 && channels != 3) OPB_FAIL(ctx, OPB_ERR_ARG, "channels must be 1 (gray) or 3 (BGR)");
+  if (!(sf > 1.0) || !std::isfinite(sf)) OPB_FAIL(ctx, OPB_ERR_ARG, "scale_factor must be a finite number > 1");
+  if (min_w < 0 || min_h < 0 || max_w < 0 || max_h < 0) OPB_FAIL(ctx, OPB_ERR_ARG, "sizes must not be negative");
+  if (h > 32767 || w > 32767) OPB_FAIL(ctx, OPB_ERR_ARG, "frame larger than 32767 pixels on a side");
+  return OPB_OK;
+}
+
+// Uploads the frame and runs the four pyramid / integral / window launches; `sums` (optional) receives stage sums.
+int cascade_run(opb_ctx* ctx, CascadeState* cs, const uint8_t* img, int img_loc, int h, int w, int channels,
+                double* sums, const uint8_t** d_frame_out) {
+  const size_t bytes = static_cast<size_t>(h) * w * channels;
+  const uint8_t* d_frame = img;
+  if (img_loc == OPB_HOST) {
+    if (cs->frame_cap < bytes) {
+      OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      cudaFree(cs->d_frame);
+      cs->d_frame = nullptr;
+      cs->frame_cap = 0;
+      OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&cs->d_frame), bytes));
+      cs->frame_cap = bytes;
+    }
+    if (int rc = copy_in(ctx, cs->d_frame, img, bytes, OPB_HOST)) return rc;
+    d_frame = cs->d_frame;
+  }
+  if (d_frame_out) *d_frame_out = d_frame;
+  if (!cs->d_cand) {
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&cs->d_cand), sizeof(int) * (1 + 3 * kCascadeMaxRaw)));
+    OPB_CUDA(ctx, cudaMallocHost(reinterpret_cast<void**>(&cs->h_cand), sizeof(int) * (1 + 3 * kCascadeMaxRaw)));
+  }
+  const int nl = static_cast<int>(cs->layers.size());
+  if (nl == 0) return OPB_OK;
+  const int P = cs->pitch;
+  cascade_pyramid_kernel<<<dim3((cs->max_w + 31) / 32, (cs->max_h + 7) / 8, nl), dim3(32, 8), 0, ctx->stream>>>(
+      d_frame, h, w, channels, cs->d_layers, cs->d_axes, cs->d_img, P, cs->d_cand);
+  cascade_row_scan_kernel<<<dim3((cs->max_h + 1 + 7) / 8, nl), dim3(32, 8), 0, ctx->stream>>>(cs->d_layers, cs->d_img, P,
+                                                                                              cs->d_sum, cs->d_sq);
+  cascade_col_scan_kernel<<<dim3((cs->max_w + 1 + 127) / 128, nl), 128, 0, ctx->stream>>>(cs->d_layers, P, cs->d_sum,
+                                                                                          cs->d_sq);
+  ctx->launches += 3;
+  OPB_CUDA(ctx, cudaGetLastError());
+  if (cs->n_windows == 0) return OPB_OK;
+  CascadeWindowSetup ws{};
+  const int nw = cs->win_w - 2, nh = cs->win_h - 2;
+  ws.nofs[0] = P + 1; ws.nofs[1] = P + 1 + nw; ws.nofs[2] = (1 + nh) * P + 1; ws.nofs[3] = (1 + nh) * P + 1 + nw;
+  ws.area = static_cast<double>(nw * nh);
+  cascade_eval_kernel<<<(cs->n_windows + 127) / 128, 128, 0, ctx->stream>>>(
+      cs->d_layers, nl, cs->n_windows, P, cs->d_sum, cs->d_sq, cs->d_stages, static_cast<int>(cs->stages.size()),
+      cs->d_stumps, static_cast<int>(cs->feat.size()), ws, cs->d_codes, sums);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  return OPB_OK;
+}
+
+struct CvRect { int x, y, w, h; };
+
+bool rect_less(const CvRect& a, const CvRect& b) {
+  if (a.y != b.y) return a.y < b.y;
+  if (a.x != b.x) return a.x < b.x;
+  if (a.w != b.w) return a.w < b.w;
+  return a.h < b.h;
+}
+
+// cv::groupRectangles(rects, group_threshold, 0.2) as detectMultiScale applies it (partition with SimilarRects,
+// float averaging, the inside-a-bigger-class filter).  The set it returns does not depend on the input order.
+std::vector<CvRect> group_rectangles(const std::vector<CvRect>& in, int thr) {
+  const double eps = 0.2;
+  if (thr <= 0 || in.empty()) return in;
+  const int n = static_cast<int>(in.size());
+  std::vector<int> parent(n);
+  for (int i = 0; i < n; ++i) parent[i] = i;
+  auto find = [&](int i) { while (parent[i] != i) { parent[i] = parent[parent[i]]; i = parent[i]; } return i; };
+  for (int i = 0; i < n; ++i)
+    for (int j = i + 1; j < n; ++j) {
+      const CvRect &a = in[i], &b = in[j];
+      const double delta = eps * (std::min(a.w, b.w) + std::min(a.h, b.h)) * 0.5;
+      if (std::abs(a.x - b.x) <= delta && std::abs(a.y - b.y) <= delta && std::abs(a.x + a.w - b.x - b.w) <= delta &&
+          std::abs(a.y + a.h - b.y - b.h) <= delta) {
+        const int ra = find(i), rb = find(j);
+        if (ra != rb) parent[rb] = ra;
+      }
+    }
+  std::map<int, int> cls;
+  std::vector<long long> sx, sy, sw, sh;
+  std::vector<int> cnt;
+  for (int i = 0; i < n; ++i) {
+    const int r = find(i);
+    auto it = cls.find(r);
+    int c;
+    if (it == cls.end()) { c = static_cast<int>(cnt.size()); cls[r] = c; sx.push_back(0); sy.push_back(0); sw.push_back(0); sh.push_back(0); cnt.push_back(0); }
+    else c = it->second;
+    sx[c] += in[i].x; sy[c] += in[i].y; sw[c] += in[i].w; sh[c] += in[i].h; cnt[c]++;
+  }
+  const int nc = static_cast<int>(cnt.size());
+  std::vector<CvRect> avg(nc);
+  for (int c = 0; c < nc; ++c) {
+    const float s = 1.f / static_cast<float>(cnt[c]);
+    avg[c] = CvRect{cv_round(static_cast<float>(sx[c]) * s), cv_round(static_cast<float>(sy[c]) * s),
+                    cv_round(static_cast<float>(sw[c]) * s), cv_round(static_cast<float>(sh[c]) * s)};
+  }
+  std::vector<CvRect> out;
+  for (int i = 0; i < nc; ++i) {
+    const CvRect r1 = avg[i];
+    const int n1 = cnt[i];
+    if (n1 <= thr) continue;
+    int j = 0;
+    for (; j < nc; ++j) {
+      const int n2 = cnt[j];
+      if (j == i || n2 <= thr) continue;
+      const CvRect r2 = avg[j];
+      const int dx = cv_round(r2.w * eps), dy = cv_round(r2.h * eps);
+      if (r1.x >= r2.x - dx && r1.y >= r2.y - dy && r1.x + r1.w <= r2.x + r2.w + dx && r1.y + r1.h <= r2.y + r2.h + dy &&
+          (n2 > std::max(3, n1) || n1 < 3))
+        break;
+    }
+    if (j == nc) out.push_back(r1);
+  }
+  return out;
+}
+
+// The full detectMultiScale: upload, five launches, one candidate download and synchronisation, host grouping.
+int cascade_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, int channels, double sf, int min_nb,
+                   int min_w, int min_h, int max_w, int max_h, std::vector<CvRect>& out, const uint8_t** d_frame) {
+  CascadeState* cs = ctx->cascade;
+  int rc;
+  if ((rc = cascade_plan(ctx, cs, h, w, sf, min_w, min_h, max_w, max_h))) return rc;
+  if ((rc = cascade_run(ctx, cs, img, img_loc, h, w, channels, nullptr, d_frame))) return rc;
+  out.clear();
+  if (cs->n_windows == 0) return OPB_OK;
+  const int nl = static_cast<int>(cs->layers.size());
+  cascade_compact_kernel<<<dim3((cs->max_ny + 3) / 4, nl), dim3(32, 4), 0, ctx->stream>>>(cs->d_layers, cs->d_codes,
+                                                                                        cs->d_cand, kCascadeMaxRaw);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  OPB_CUDA(ctx, cudaMemcpyAsync(cs->h_cand, cs->d_cand, sizeof(int) * (1 + 3 * kCascadeMaxRaw), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  const int n = cs->h_cand[0];
+  if (n > kCascadeMaxRaw) OPB_FAIL(ctx, OPB_ERR_CAPACITY, "more than 8192 raw cascade candidates in one frame");
+  std::vector<CvRect> raw(n);
+  for (int i = 0; i < n; ++i) {
+    const CascadeLayer& L = cs->layers[cs->h_cand[1 + 3 * i]];
+    const float s = L.scale;
+    const int x = cv_round(static_cast<float>(cs->h_cand[2 + 3 * i]) * s);
+    const int y = cv_round(static_cast<float>(cs->h_cand[3 + 3 * i]) * s);
+    const int rw = cv_round(static_cast<float>(cs->win_w) * s), rh = cv_round(static_cast<float>(cs->win_h) * s);
+    raw[i] = CvRect{x, y, std::min(x + rw, w) - x, std::min(y + rh, h) - y};   // clipped to the frame, as cv2 4.13
+  }
+  out = group_rectangles(raw, min_nb);
+  std::sort(out.begin(), out.end(), rect_less);
+  return OPB_OK;
+}
+
+int cascade_write_rects(opb_ctx* ctx, const std::vector<CvRect>& r, int32_t* rects_out, int cap, int* n_out) {
+  *n_out = static_cast<int>(r.size());
+  if (static_cast<int>(r.size()) > cap) OPB_FAIL(ctx, OPB_ERR_CAPACITY, "more detections than rects_out holds");
+  for (size_t i = 0; i < r.size(); ++i) {
+    rects_out[i * 4 + 0] = r[i].x; rects_out[i * 4 + 1] = r[i].y; rects_out[i * 4 + 2] = r[i].w; rects_out[i * 4 + 3] = r[i].h;
+  }
+  return OPB_OK;
+}
+
+}  // namespace
+
+int opb_cascade_load(opb_ctx* ctx, int win_w, int win_h, int n_stages, const int32_t* stage_ntrees,
+                     const float* stage_threshold, int n_stumps, const int32_t* stump_feature,
+                     const float* stump_threshold, const float* stump_left, const float* stump_right, int n_features,
+                     const int32_t* rects, const float* weights) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (win_w < 3 || win_h < 3 || win_w > 1024 || win_h > 1024) OPB_FAIL(ctx, OPB_ERR_ARG, "window size out of range");
+  if (n_stages <= 0 || n_stages > kCascadeMaxStages) OPB_FAIL(ctx, OPB_ERR_ARG, "stage count must be in [1, 64]");
+  if (n_stumps <= 0 || n_features <= 0 || !stage_ntrees || !stage_threshold || !stump_feature || !stump_threshold ||
+      !stump_left || !stump_right || !rects || !weights)
+    OPB_FAIL(ctx, OPB_ERR_ARG, "empty or missing cascade tables");
+  auto cs = std::unique_ptr<CascadeState>(new CascadeState());
+  cs->win_w = win_w; cs->win_h = win_h;
+  long long first = 0;
+  for (int s = 0; s < n_stages; ++s) {
+    if (stage_ntrees[s] <= 0) OPB_FAIL(ctx, OPB_ERR_ARG, "a stage without stumps");
+    cs->stages.push_back(CascadeStage{static_cast<int>(first), stage_ntrees[s], stage_threshold[s] - kCascadeThresholdEps, 0});
+    first += stage_ntrees[s];
+  }
+  if (first != n_stumps) OPB_FAIL(ctx, OPB_ERR_ARG, "stage tree counts do not add up to the stump count");
+  for (int t = 0; t < n_stumps; ++t)
+    if (stump_feature[t] < 0 || stump_feature[t] >= n_features) OPB_FAIL(ctx, OPB_ERR_ARG, "stump feature index out of range");
+  for (int f = 0; f < n_features; ++f)
+    for (int r = 0; r < 3; ++r) {
+      const int32_t* q = rects + (static_cast<size_t>(f) * 3 + r) * 4;
+      if (weights[f * 3 + r] == 0.f && r > 0) continue;
+      if (q[0] < 0 || q[1] < 0 || q[2] < 0 || q[3] < 0 || q[0] + q[2] > win_w || q[1] + q[3] > win_h)
+        OPB_FAIL(ctx, OPB_ERR_ARG, "feature " + std::to_string(f) + " has a rect outside the window");
+    }
+  cs->feat.assign(stump_feature, stump_feature + n_stumps);
+  cs->sthr.assign(stump_threshold, stump_threshold + n_stumps);
+  cs->sleft.assign(stump_left, stump_left + n_stumps);
+  cs->sright.assign(stump_right, stump_right + n_stumps);
+  cs->rects.assign(rects, rects + static_cast<size_t>(n_features) * 12);
+  cs->weights.assign(weights, weights + static_cast<size_t>(n_features) * 3);
+  for (int f = 0; f < n_features; ++f)     // an absent rect reads nothing: point it at the window origin
+    for (int r = 1; r < 3; ++r)
+      if (cs->weights[f * 3 + r] == 0.f) std::fill_n(&cs->rects[(static_cast<size_t>(f) * 3 + r) * 4], 4, 0);
+  cudaSetDevice(ctx->device);
+  OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&cs->d_stages), sizeof(CascadeStage) * n_stages));
+  OPB_CUDA(ctx, cudaMemcpyAsync(cs->d_stages, cs->stages.data(), sizeof(CascadeStage) * n_stages, cudaMemcpyHostToDevice,
+                                ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  delete ctx->cascade;
+  ctx->cascade = cs.release();
+  return OPB_OK;
+}
+
+int opb_cascade_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, int channels, double scale_factor,
+                       int min_neighbors, int min_w, int min_h, int max_w, int max_h, int32_t* rects_out, int cap,
+                       int* n_out) {
+  if (!ctx) return OPB_ERR_ARG;
+  int rc;
+  if ((rc = cascade_check(ctx, img, h, w, channels, scale_factor, min_w, min_h, max_w, max_h))) return rc;
+  if (min_neighbors < 0 || cap < 0 || !n_out || (cap > 0 && !rects_out)) OPB_FAIL(ctx, OPB_ERR_ARG, "bad output or min_neighbors");
+  cudaSetDevice(ctx->device);
+  std::vector<CvRect> r;
+  if ((rc = cascade_detect(ctx, img, img_loc, h, w, channels, scale_factor, min_neighbors, min_w, min_h, max_w, max_h, r,
+                           nullptr)))
+    return rc;
+  return cascade_write_rects(ctx, r, rects_out, cap, n_out);
+}
+
+int opb_face_detect_frame(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int h, int w, double scale_factor,
+                          int min_neighbors, int min_w, int min_h, int max_w, int max_h, double crop_scale,
+                          int net_size, double thresh, int32_t* rects_out, int cap, int* n_out, double* out,
+                          int32_t* valid, int32_t* left_top) {
+  if (!ctx) return OPB_ERR_ARG;
+  int rc;
+  if ((rc = cascade_check(ctx, frame, h, w, 3, scale_factor, min_w, min_h, max_w, max_h))) return rc;
+  if (!ctx->kp_out) OPB_FAIL(ctx, OPB_ERR_STATE, "this context holds the pose net: load FaceNet weights first");
+  if (min_neighbors < 0 || cap < 0 || !n_out || (cap > 0 && (!rects_out || !out || !valid || !left_top)))
+    OPB_FAIL(ctx, OPB_ERR_ARG, "bad output or min_neighbors");
+  if (!(crop_scale > 0.0) || !std::isfinite(crop_scale)) OPB_FAIL(ctx, OPB_ERR_ARG, "crop_scale must be positive");
+  if (net_size <= 0 || net_size % 8) OPB_FAIL(ctx, OPB_ERR_ARG, "net_size must be a positive multiple of 8");
+  cudaSetDevice(ctx->device);
+  std::vector<CvRect> r;
+  const uint8_t* d_frame = nullptr;
+  if ((rc = cascade_detect(ctx, frame, frame_loc, h, w, 3, scale_factor, min_neighbors, min_w, min_h, max_w, max_h, r,
+                           &d_frame)))
+    return rc;
+  if ((rc = cascade_write_rects(ctx, r, rects_out, cap, n_out))) return rc;
+  if (r.empty()) return OPB_OK;
+  // crop_face of camera_face_demo.py:10-24: int() truncates toward zero; right / bottom clamp to w / h; the crop is
+  // zero-padded at the bottom and right to an edge x edge square
+  std::vector<KpCrop> table(r.size());
+  for (size_t i = 0; i < r.size(); ++i) {
+    const double cx = r[i].x + r[i].w / 2.0, cy = r[i].y + r[i].h / 2.0;
+    const double cw = r[i].w * crop_scale, chh = r[i].h * crop_scale;
+    const int left = std::max(0, static_cast<int>(cx - cw / 2)), top = std::max(0, static_cast<int>(cy - chh / 2));
+    const int right = std::min(w, static_cast<int>(cx + cw / 2)), bottom = std::min(h, static_cast<int>(cy + chh / 2));
+    if (right <= left || bottom <= top) OPB_FAIL(ctx, OPB_ERR_ARG, "a face rect gives an empty crop");
+    KpCrop& c = table[i];
+    c.top = top; c.left = left; c.vh = bottom - top; c.vw = right - left;
+    c.h = c.w = std::max(c.vh, c.vw);
+    c.flip = 0;
+    left_top[i * 2 + 0] = left;
+    left_top[i * 2 + 1] = top;
+  }
+  return kp_detect_table(ctx, d_frame, h, w, table, net_size, thresh, out, valid);
+}
+
+int opb_test_cascade_windows(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, int channels,
+                             double scale_factor, int min_w, int min_h, int max_w, int max_h, int32_t* codes_out,
+                             double* sums_out, int cap, int* n_out) {
+  if (!ctx) return OPB_ERR_ARG;
+  int rc;
+  if ((rc = cascade_check(ctx, img, h, w, channels, scale_factor, min_w, min_h, max_w, max_h))) return rc;
+  if (!n_out || cap < 0 || (cap > 0 && (!codes_out || !sums_out))) OPB_FAIL(ctx, OPB_ERR_ARG, "bad output");
+  cudaSetDevice(ctx->device);
+  CascadeState* cs = ctx->cascade;
+  if ((rc = cascade_plan(ctx, cs, h, w, scale_factor, min_w, min_h, max_w, max_h))) return rc;
+  *n_out = cs->n_windows;
+  if (cs->n_windows > cap) OPB_FAIL(ctx, OPB_ERR_CAPACITY, "more windows than the output holds");
+  if (cs->sums_cap < static_cast<size_t>(cs->n_windows)) {
+    OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(cs->d_sums);
+    cs->d_sums = nullptr;
+    cs->sums_cap = 0;
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&cs->d_sums), sizeof(double) * std::max(cs->n_windows, 1)));
+    cs->sums_cap = cs->n_windows;
+  }
+  if ((rc = cascade_run(ctx, cs, img, img_loc, h, w, channels, cs->d_sums, nullptr))) return rc;
+  if (cs->n_windows == 0) return OPB_OK;
+  if ((rc = copy_out(ctx, codes_out, cs->d_codes, sizeof(int) * cs->n_windows, OPB_HOST))) return rc;
+  if ((rc = copy_out(ctx, sums_out, cs->d_sums, sizeof(double) * cs->n_windows, OPB_HOST))) return rc;
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return OPB_OK;
 }
 
 void* opb_device_buffer(opb_ctx* ctx, int which) {

@@ -50,6 +50,20 @@ class FaceDetector(object):
         return self.engine.keypoints_detect_crops(img, table, params["face_inference_img_size"],
                                                   params['face_heatmap_peak_thresh'])
 
+    def detect_frame(self, img, cascade, scaleFactor=1.2, minNeighbors=3, minSize=(1, 1), maxSize=(0, 0)):
+        """The per-frame work of camera_face_demo.py:47-56 in one device call (opb_face_detect_frame): the Haar cascade
+        (`cascade`: a cascade.CascadeClassifier) on `img` (uint8 BGR [H,W,3]), then FaceNet on the demo's crop_face of
+        every face.  Returns (facerects, [(keypoints, (crop_left, crop_top)), ...]): facerects as
+        cascade.detectMultiScale returns them (sorted by (y, x, w, h), () when empty), keypoints as
+        self(crop_face(img, rect)[0]) of that demo."""
+        if getattr(self.engine, "cascade_tables", None) is not cascade.tables:
+            self.engine.cascade_load(cascade.tables)
+        rects, kps, left_top = self.engine.face_detect_frame(img, scaleFactor, minNeighbors, minSize, maxSize,
+                                                             params['face_crop_scale'],
+                                                             params["face_inference_img_size"],
+                                                             params['face_heatmap_peak_thresh'])
+        return (rects if len(rects) else ()), list(zip(kps, left_top))
+
     def create_gaussian_kernel(self, sigma=1, ksize=5):
         """The 2-D kernel of the reference's GPU branch (face_detector.py:44-52); kept for API compatibility --
         peak extraction here follows the CPU branch (scipy gaussian_filter) exactly."""

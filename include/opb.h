@@ -293,6 +293,44 @@ int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc
                                const opb_crop* crops, int n, int net_size, double thresh,
                                double* out /* [n][C-1][3] */, int32_t* valid /* [n][C-1] */);
 
+/* ---- Haar cascade (cv2.CascadeClassifier.detectMultiScale, stump-based HAAR cascades, bit-exact) ----
+ * opb_cascade_load: one cascade per context (a second load replaces the first).  Flat tables as the XML holds them:
+ *   stage_ntrees / stage_threshold [n_stages] (stageThreshold as stored; the 1e-5f margin is applied here),
+ *   stump_feature / stump_threshold / stump_left / stump_right [n_stumps] stage by stage,
+ *   rects [n_features][3][4] (x, y, w, h; unused rects zero) and weights [n_features][3] (0: rect absent).
+ *   OPB_ERR_ARG for a rect outside the window, a feature index out of range, ntrees that do not add up to n_stumps,
+ *   or more than 64 stages. */
+int opb_cascade_load(opb_ctx* ctx, int win_w, int win_h, int n_stages, const int32_t* stage_ntrees,
+                     const float* stage_threshold, int n_stumps, const int32_t* stump_feature,
+                     const float* stump_threshold, const float* stump_left, const float* stump_right, int n_features,
+                     const int32_t* rects, const float* weights);
+/* opb_cascade_detect: detectMultiScale(gray, scale_factor, min_neighbors, (min_w, min_h), (max_w, max_h)) of an
+ *   h x w frame with channels 1 (gray) or 3 (BGR, converted as cvtColor(BGR2GRAY)).  rects_out [cap][4] (x, y, w, h)
+ *   sorted by (y, x, w, h).  Per call: one frame upload, five launches (pyramid, row scan, column scan, windows,
+ *   compaction), one candidate download and one synchronisation; grouping runs on the host.  Per-shape tables are
+ *   uploaded on the first call of a shape.  OPB_ERR_ARG (nothing enqueued) for scale_factor <= 1, a negative
+ *   argument or channels other than 1 and 3; OPB_ERR_STATE without a cascade; OPB_ERR_CAPACITY when the result
+ *   (or the raw candidate list, 8192 entries) does not fit, never truncation. */
+int opb_cascade_detect(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, int channels, double scale_factor,
+                       int min_neighbors, int min_w, int min_h, int max_w, int max_h, int32_t* rects_out, int cap,
+                       int* n_out);
+/* opb_face_detect_frame: the per-frame work of camera_face_demo.py:47-56 -- the cascade on the BGR frame, then for
+ *   every face rect its zero-padded square crop (crop_face of that demo, scaled by crop_scale), FaceNet on all crops
+ *   in the chunks of opb_keypoints_detect_crops, and the keypoints.  rects_out as opb_cascade_detect; out [cap][C-1][3]
+ *   and valid [cap][C-1] as opb_keypoints_detect_crops, in crop coordinates; left_top [cap][2] = (crop_left,
+ *   crop_top).  Per call: one frame upload, one candidate download and synchronisation, one crop-table upload, one
+ *   keypoint download and synchronisation.  Errors as opb_cascade_detect, and OPB_ERR_STATE without FaceNet. */
+int opb_face_detect_frame(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int h, int w, double scale_factor,
+                          int min_neighbors, int min_w, int min_h, int max_w, int max_h, double crop_scale,
+                          int net_size, double thresh, int32_t* rects_out, int cap, int* n_out, double* out,
+                          int32_t* valid, int32_t* left_top);
+/* Test hook: the result code (-1 variance test failed, -k rejected by stage k, 1 passed) and final stage sum of every
+ *   window of every scale, before the skip rule: layers in scale order, windows row by row (y, x in the layer's
+ *   ystep).  *n_out = number of windows; OPB_ERR_CAPACITY when it exceeds cap. */
+int opb_test_cascade_windows(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, int channels,
+                             double scale_factor, int min_w, int min_h, int max_w, int max_h, int32_t* codes_out,
+                             double* sums_out, int cap, int* n_out);
+
 /* device pointers of the last opb_detect_batch outputs/intermediates (valid until the next
  * call with a different shape): 0 paf_lo, 1 heat_lo, 2 pafs (full-res), 3 heatmaps (full-res),
  * 4 headers, 5 persons, 6 peak table ([N,max_peaks] of {int32 type,x,y; float score})       */
