@@ -36,9 +36,12 @@ CROP_DTYPE = np.dtype([("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bott
 PART_DTYPE = np.dtype([("kind", "<i4"), ("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bottom", "<i4"),
                        ("first_point", "<i4")])   # opb_part
 PART_FACE, PART_HAND = 0, 1
+WB_PART_DTYPE = np.dtype([("kind", "<i4"), ("left", "<i4"), ("top", "<i4"), ("right", "<i4"), ("bottom", "<i4"),
+                          ("row", "<i4"), ("person", "<i4"), ("side", "<i4")])   # opb_wb_part
+SIDE_FACE, SIDE_LEFT, SIDE_RIGHT = 0, 1, 2
 PART_POINTS = {PART_FACE: 70, PART_HAND: 21}
 assert PERSON_DTYPE.itemsize == 240 and HEADER_DTYPE.itemsize == 16 and CROP_DTYPE.itemsize == 24
-assert PART_DTYPE.itemsize == 24
+assert PART_DTYPE.itemsize == 24 and WB_PART_DTYPE.itemsize == 32
 
 
 def crop_table(bboxes, flips=None):
@@ -146,6 +149,12 @@ _SIGNATURES = {
     "opb_test_cascade_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
                                            C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                            C.POINTER(C.c_int)]),
+    "opb_whole_body_frame": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.c_double, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "opb_test_whole_body_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
 }
 
 _lib = None
@@ -194,6 +203,7 @@ class Engine(object):
             self.ctx = None
             raise OpbError("opb_create failed (%d): %s" % (rc, msg.decode() if msg else "?"))
         self.precision = precision
+        self.device = int(device)
         self._weights_ready = False
 
     def __del__(self):
@@ -666,6 +676,50 @@ class Engine(object):
         k = n.value
         return (rects[:k].copy(), [self._keypoint_list(o, v) for o, v in zip(out[:k], valid[:k])],
                 [(int(a), int(b)) for a, b in left_top[:k]])
+
+    # -- the whole-body frame (include/opb.h: opb_whole_body_frame) ---------------------------------
+    def whole_body_frame(self, face_engine, hand_engine, img, in_h, in_w, map_h, map_w, img_len, face_net_size,
+                         face_thresh, hand_net_size, hand_thresh, draw=True, inject_paf=None, inject_heat=None):
+        """demo.py's frame on the device with this (pose) context and the FaceNet / HandNet contexts: returns
+        (headers[1], persons[1, max_persons], parts (WB_PART_DTYPE [n]), face keypoint lists by row, hand keypoint lists
+        by row, picture [H,W,3] uint8 or None).  inject_*: device pointers (ints) or None, as in detect_batch."""
+        img = np.ascontiguousarray(img, np.uint8)
+        oh, ow, _ = img.shape
+        headers = np.empty(1, HEADER_DTYPE)
+        persons = np.empty((1, self.max_persons), PERSON_DTYPE)
+        cap = 3 * self.max_persons                     # every person has at most a face and two hands
+        parts = np.empty(cap, WB_PART_DTYPE)
+        fpl = max(getattr(face_engine, "kp_channels", 0) - 1, 0)
+        hpl = max(getattr(hand_engine, "kp_channels", 0) - 1, 0)
+        face_out, face_valid = np.empty((cap, fpl, 3), np.float64), np.empty((cap, fpl), np.int32)
+        hand_out, hand_valid = np.empty((cap, hpl, 3), np.float64), np.empty((cap, hpl), np.int32)
+        picture = np.empty_like(img) if draw else None
+        n = C.c_int(0)
+        self._check(self.lib.opb_whole_body_frame(
+            self.ctx, face_engine.ctx, hand_engine.ctx, _ptr(img), OPB_HOST, oh, ow, in_h, in_w, map_h, map_w,
+            float(img_len), C.c_void_p(int(inject_paf)) if inject_paf else None,
+            C.c_void_p(int(inject_heat)) if inject_heat else None, int(face_net_size), float(face_thresh),
+            int(hand_net_size), float(hand_thresh), _ptr(headers), _ptr(persons), _ptr(parts), cap, C.byref(n),
+            _ptr(face_out), _ptr(face_valid), _ptr(hand_out), _ptr(hand_valid), _ptr(picture)))
+        parts = parts[:n.value].copy()
+        n_face = int((parts["kind"] == PART_FACE).sum())
+        faces = [self._keypoint_list(o, v) for o, v in zip(face_out[:n_face], face_valid[:n_face])]
+        hands = [self._keypoint_list(o, v) for o, v in zip(hand_out[:n.value - n_face], hand_valid[:n.value - n_face])]
+        return headers, persons, parts, faces, hands, picture
+
+    def test_whole_body_boxes(self, persons, sx, sy):
+        """Test hook: the crop-box kernel on host person records (PERSON_DTYPE [n]) -> (unit lengths float64 [n],
+        boxes int32 [n, 3, 4] (face, left, right), present bits int32 [n], kept parts int32 [k, 2] (person, side))."""
+        rec = np.ascontiguousarray(persons, PERSON_DTYPE)
+        n = len(rec)
+        unit = np.empty(max(n, 1), np.float64)
+        boxes = np.zeros((max(n, 1), 3, 4), np.int32)
+        present = np.empty(max(n, 1), np.int32)
+        parts = np.empty((3 * max(n, 1), 2), np.int32)
+        k = C.c_int(0)
+        self._check(self.lib.opb_test_whole_body_boxes(self.ctx, _ptr(rec), n, float(sx), float(sy), _ptr(unit),
+                                                       _ptr(boxes), _ptr(present), _ptr(parts), C.byref(k)))
+        return unit[:n], boxes[:n], present[:n], parts[:k.value].copy()
 
     def test_cascade_windows(self, img, scale_factor, min_size=(0, 0), max_size=(0, 0)):
         """Test hook: (codes int32 [n], stage sums float64 [n]) of every window of every scale, before the skip rule."""

@@ -30,6 +30,7 @@
 #include "peaks_sep.cuh"
 #include "pool.cuh"
 #include "upsample.cuh"
+#include "whole_body.cuh"
 
 using namespace opb;
 
@@ -38,6 +39,8 @@ static_assert(sizeof(opb_person) == 240, "opb_person size");
 static_assert(sizeof(opb_image_header) == sizeof(ImageHeader), "opb_image_header layout");
 static_assert(sizeof(opb_crop) == 24, "opb_crop size");
 static_assert(sizeof(opb_part) == 24, "opb_part size");
+static_assert(sizeof(opb_wb_part) == 32, "opb_wb_part size");
+static_assert(sizeof(opb_crop) == sizeof(WbCrop), "opb_crop layout");
 
 namespace {
 
@@ -170,6 +173,9 @@ struct opb_ctx {
   float* precise_mid = nullptr;    // x8 cubic intermediate of the precise path
   uint8_t* ov_buf = nullptr;       // overlay scratch: [frame in | frame out | priority plane | int poses | flag]
   size_t ov_bytes = 0;
+  uint8_t* wb_buf = nullptr;       // opb_whole_body_frame: box-kernel outputs (whole_body.cuh) ...
+  uint8_t* wb_host = nullptr;      // ... and their pinned host copy, preceded by the record block
+  size_t wb_bytes = 0, wb_host_bytes = 0;
   size_t precise_mid_cap = 0;
   size_t ingest_bytes = 0;
   // streaming mode (opb_stream_submit / opb_stream_collect): two slots, pinned staging, a copy stream
@@ -1158,6 +1164,8 @@ void opb_destroy(opb_ctx* ctx) {
   if (ctx->ingest_buf) cudaFree(ctx->ingest_buf);
   if (ctx->precise_mid) cudaFree(ctx->precise_mid);
   if (ctx->ov_buf) cudaFree(ctx->ov_buf);
+  if (ctx->wb_buf) cudaFree(ctx->wb_buf);
+  if (ctx->wb_host) cudaFreeHost(ctx->wb_host);
   if (ctx->kp_ws) {
     cudaFree(ctx->kp_ws->up); cudaFree(ctx->kp_ws->tmp); cudaFree(ctx->kp_ws->res); cudaFreeHost(ctx->kp_ws->h_res);
     cudaFree(ctx->kp_ws->crops);
@@ -1933,22 +1941,9 @@ int opb_draw_last_result(opb_ctx* ctx, int image_index, const uint8_t* img, int 
                      ws->persons + static_cast<size_t>(image_index) * ctx->prm.max_persons, sx, sy, out, out_loc);
 }
 
-// ---- the whole-body picture of demo.py:28-57 on the device (face_detector.py:79-97, hand_detector.py:89-117;
-// csrc/overlay.cuh): one upload of the frame and of the tables, one raster and one paint launch, one download
-int opb_draw_whole_body(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, const int32_t* poses, int n_poses,
-                        const opb_part* parts, int n_parts, const int32_t* points, int n_points, uint8_t* out, int out_loc) {
-  if (!ctx) return OPB_ERR_ARG;
-  if (!img || !out || h <= 0 || w <= 0 || n_poses < 0 || n_parts < 0 || n_points < 0 || (n_poses > 0 && !poses) ||
-      (n_parts > 0 && !parts) || (n_points > 0 && !points))
-    OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: bad image, pose, part or point arguments");
-  const long long n_prim = static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) + static_cast<long long>(n_parts) * OV_PART_STRIDE;
-  if (n_prim > (1ll << 30)) OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: too many poses / parts");
-  // the raster kernel reads everything below without bounds checks: validate it all before anything is enqueued
-  for (long long k = 0; k < static_cast<long long>(n_poses) * OV_JOINTS; ++k) {
-    const int32_t* a = poses + 3 * k;
-    if (a[2] != 0 && (a[0] < 0 || a[0] >= w || a[1] < 0 || a[1] >= h))
-      OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a joint lies outside the image");
-  }
+// Every part's kind, point range, box and present keypoints checked before the raster kernel reads them unchecked:
+// OPB_ERR_ARG for an unknown kind, points past n_points, or a box or drawn keypoint coordinate beyond 2^20.
+static int check_parts(opb_ctx* ctx, const opb_part* parts, int n_parts, const int32_t* points, int n_points) {
   auto big = [](long long v) { return v < -(1ll << 20) || v > (1ll << 20); };   // keeps the rasterisers' ints in range
   for (int p = 0; p < n_parts; ++p) {
     const opb_part& pt = parts[p];
@@ -1965,13 +1960,33 @@ int opb_draw_whole_body(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, in
         OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a keypoint coordinate exceeds 2^20 in magnitude");
     }
   }
+  return OPB_OK;
+}
+
+// ---- the whole-body picture of demo.py:28-57 on the device (face_detector.py:79-97, hand_detector.py:89-117;
+// csrc/overlay.cuh): one upload of the frame and of the tables, one raster and one paint launch, one download
+int opb_draw_whole_body(opb_ctx* ctx, const uint8_t* img, int img_loc, int h, int w, const int32_t* poses, int n_poses,
+                        const opb_part* parts, int n_parts, const int32_t* points, int n_points, uint8_t* out, int out_loc) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (!img || !out || h <= 0 || w <= 0 || n_poses < 0 || n_parts < 0 || n_points < 0 || (n_poses > 0 && !poses) ||
+      (n_parts > 0 && !parts) || (n_points > 0 && !points))
+    OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: bad image, pose, part or point arguments");
+  const long long n_prim = static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) + static_cast<long long>(n_parts) * OV_PART_STRIDE;
+  if (n_prim > (1ll << 30)) OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: too many poses / parts");
+  // the raster kernel reads everything below without bounds checks: validate it all before anything is enqueued
+  for (long long k = 0; k < static_cast<long long>(n_poses) * OV_JOINTS; ++k) {
+    const int32_t* a = poses + 3 * k;
+    if (a[2] != 0 && (a[0] < 0 || a[0] >= w || a[1] < 0 || a[1] >= h))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "draw_whole_body: a joint lies outside the image");
+  }
+  int rc;
+  if ((rc = check_parts(ctx, parts, n_parts, points, n_points))) return rc;
   cudaSetDevice(ctx->device);
   // scratch: [frame in | frame out | priority plane | tables: int poses | parts | points]
   const size_t px = static_cast<size_t>(h) * w, img_b = (px * 3 + 255) & ~size_t(255), prio_b = (px * 4 + 255) & ~size_t(255);
   const size_t poses_n = static_cast<size_t>(n_poses) * OV_JOINTS * 3, parts_n = static_cast<size_t>(n_parts) * 6;
   const size_t tab_n = poses_n + parts_n + static_cast<size_t>(n_points) * 3;
   static_assert(sizeof(opb_part) == 6 * sizeof(int32_t) && sizeof(OvPart) == sizeof(opb_part), "opb_part layout");
-  int rc;
   if ((rc = ov_reserve(ctx, 2 * img_b + prio_b + tab_n * 4 + 256))) return rc;
   uint8_t* d_in = ctx->ov_buf;
   uint8_t* d_out = ctx->ov_buf + img_b;
@@ -2359,10 +2374,9 @@ static void kp_records_to_keypoints(const ChannelMax* res, int planes, int W, do
   }
 }
 
-// Smooths the ragged maps in ws->up (both passes) and takes every (crop, plane) maximum; one copy of the records to
-// the host, one synchronisation, then the host conversion.  ws->crops must already hold `table`.
-static int kp_peaks(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, int planes, int tiles, double thresh,
-                    double* out, int32_t* valid) {
+// Smooths the ragged maps in ws->up (both passes), takes every (crop, plane) maximum and enqueues the copy of the
+// records to the pinned ws->h_res, without waiting.  ws->crops must already hold `table`.
+static int kp_peaks_enqueue(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, int planes, int tiles) {
   const int n = static_cast<int>(table.size());
   dim3 block(32, 8), grid(tiles, planes);
   gauss_pass_ragged_kernel<0><<<grid, block, 0, ctx->stream>>>(ws->up, ws->tmp, ws->crops, n, ctx->taps);
@@ -2371,11 +2385,24 @@ static int kp_peaks(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, in
   ctx->launches += 3;
   OPB_CUDA(ctx, cudaGetLastError());
   OPB_CUDA(ctx, cudaMemcpyAsync(ws->h_res, ws->res, sizeof(ChannelMax) * planes * n, cudaMemcpyDeviceToHost, ctx->stream));
-  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int i = 0; i < n; ++i)
-    kp_records_to_keypoints(ws->h_res + static_cast<size_t>(i) * planes, planes, table[i].w, thresh,
-                            out + static_cast<size_t>(i) * planes * 3, valid + static_cast<size_t>(i) * planes);
   return OPB_OK;
+}
+
+// Waits for the records kp_peaks_enqueue asked for (one synchronisation), then the host conversion.
+static int kp_peaks_collect(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, int planes, double thresh,
+                            double* out, int32_t* valid) {
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (size_t i = 0; i < table.size(); ++i)
+    kp_records_to_keypoints(ws->h_res + i * planes, planes, table[i].w, thresh, out + i * planes * 3,
+                            valid + i * planes);
+  return OPB_OK;
+}
+
+// Both halves: one copy of the records to the host, one synchronisation, then the host conversion.
+static int kp_peaks(opb_ctx* ctx, KpWs* ws, const std::vector<KpCrop>& table, int planes, int tiles, double thresh,
+                    double* out, int32_t* valid) {
+  int rc = kp_peaks_enqueue(ctx, ws, table, planes, tiles);
+  return rc ? rc : kp_peaks_collect(ctx, ws, table, planes, thresh, out, valid);
 }
 
 // Workspace and device crop table for the single-crop entry points: one [planes][h][w] map set at offset 0.
@@ -2450,9 +2477,9 @@ static int kp_chunk_slots(int remaining) {
 
 // Crops of `table` (top, left, h, w, flip, vh, vw set) of a frame already on the device, through FaceNet / HandNet in
 // chunks of kp_chunk_slots: one crop-table upload, then per chunk a crop + resize launch, the chain and a ragged
-// upsample; then kp_peaks (one download, one synchronisation).  Keypoints of crop i in crop i's canvas coordinates.
-static int kp_detect_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, int frame_w, std::vector<KpCrop>& table,
-                           int net_size, double thresh, double* out, int32_t* valid) {
+// upsample; then kp_peaks_enqueue.  Nothing waits: kp_peaks_collect(ctx, ctx->kp_ws, table, ...) collects the result.
+static int kp_enqueue_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, int frame_w, std::vector<KpCrop>& table,
+                            int net_size) {
   const int n = static_cast<int>(table.size());
   const int planes = ctx->kp_out - 1;              // the last channel is background (face_detector.py:59)
   for (KpCrop& c : table) {
@@ -2492,7 +2519,15 @@ static int kp_detect_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, in
     OPB_CUDA(ctx, cudaGetLastError());
     first += nc;
   }
-  return kp_peaks(ctx, ws, table, planes, tiles, thresh, out, valid);
+  return kp_peaks_enqueue(ctx, ws, table, planes, tiles);
+}
+
+// kp_enqueue_table, then kp_peaks_collect (one download, one synchronisation).  Keypoints of crop i in crop i's canvas
+// coordinates.
+static int kp_detect_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, int frame_w, std::vector<KpCrop>& table,
+                           int net_size, double thresh, double* out, int32_t* valid) {
+  int rc = kp_enqueue_table(ctx, d_frame, frame_h, frame_w, table, net_size);
+  return rc ? rc : kp_peaks_collect(ctx, ctx->kp_ws, table, ctx->kp_out - 1, thresh, out, valid);
 }
 
 int opb_keypoints_detect_crops(opb_ctx* ctx, const uint8_t* frame, int frame_loc, int frame_h, int frame_w,
@@ -2969,6 +3004,274 @@ int opb_test_cascade_windows(opb_ctx* ctx, const uint8_t* img, int img_loc, int 
   if ((rc = copy_out(ctx, codes_out, cs->d_codes, sizeof(int) * cs->n_windows, OPB_HOST))) return rc;
   if ((rc = copy_out(ctx, sums_out, cs->d_sums, sizeof(double) * cs->n_windows, OPB_HOST))) return rc;
   OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return OPB_OK;
+}
+
+// ---------------------------------------------------------------- the whole-body frame of demo.py (csrc/whole_body.cuh)
+namespace {
+
+// Device block of the box kernel's outputs for `cap` persons, in the order the frame call downloads it: the counts and
+// the three compacted tables first, then the per-person unit lengths, boxes and present bits (test hook only).
+struct WbLayout {
+  size_t counts, face, hand, parts, tables_end, unit, box, present, total;
+};
+
+WbLayout wb_layout(int cap) {
+  auto al = [](size_t v) { return (v + 255) & ~size_t(255); };
+  const size_t c = static_cast<size_t>(cap);
+  WbLayout L;
+  L.counts = 0;
+  L.face = al(sizeof(WbCounts));
+  L.hand = L.face + al(sizeof(WbCrop) * c);
+  L.parts = L.hand + al(sizeof(WbCrop) * 2 * c);
+  L.tables_end = L.parts + al(sizeof(WbPart) * 3 * c);
+  L.unit = L.tables_end;
+  L.box = L.unit + al(sizeof(double) * c);
+  L.present = L.box + al(sizeof(int) * 12 * c);
+  L.total = L.present + al(sizeof(int) * c);
+  return L;
+}
+
+// Grows ctx->wb_buf to the layout of `cap` persons plus `extra` bytes after it, and the pinned ctx->wb_host to
+// `host_bytes`.
+int wb_reserve(opb_ctx* ctx, int cap, size_t extra, size_t host_bytes, WbOut* out) {
+  const WbLayout L = wb_layout(cap);
+  if (ctx->wb_bytes < L.total + extra) {
+    if (ctx->wb_buf) { OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->wb_buf); ctx->wb_buf = nullptr; }
+    ctx->wb_bytes = 0;
+    OPB_CUDA(ctx, cudaMalloc(reinterpret_cast<void**>(&ctx->wb_buf), L.total + extra));
+    ctx->wb_bytes = L.total + extra;
+  }
+  if (ctx->wb_host_bytes < host_bytes) {
+    if (ctx->wb_host) { cudaFreeHost(ctx->wb_host); ctx->wb_host = nullptr; }
+    ctx->wb_host_bytes = 0;
+    OPB_CUDA(ctx, cudaMallocHost(reinterpret_cast<void**>(&ctx->wb_host), host_bytes));
+    ctx->wb_host_bytes = host_bytes;
+  }
+  uint8_t* b = ctx->wb_buf;
+  out->counts = reinterpret_cast<WbCounts*>(b + L.counts);
+  out->face = reinterpret_cast<WbCrop*>(b + L.face);
+  out->hand = reinterpret_cast<WbCrop*>(b + L.hand);
+  out->parts = reinterpret_cast<WbPart*>(b + L.parts);
+  out->unit = reinterpret_cast<double*>(b + L.unit);
+  out->box = reinterpret_cast<int*>(b + L.box);
+  out->present = reinterpret_cast<int*>(b + L.present);
+  return OPB_OK;
+}
+
+int wb_launch(opb_ctx* ctx, const ImageHeader* d_hd, const PersonOut* d_persons, int cap, double sx, double sy,
+              const WbOut& out) {
+  whole_body_boxes_kernel<<<1, WB_THREADS, 0, ctx->stream>>>(d_hd, d_persons, cap, sx, sy, out);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  return OPB_OK;
+}
+
+// opb_crop rows -> the KpCrop table of opb_keypoints_detect_crops
+int wb_kp_table(opb_ctx* ctx, const WbCrop* crops, int n, std::vector<KpCrop>& table) {
+  table.assign(n, KpCrop{});
+  for (int i = 0; i < n; ++i) {
+    const WbCrop& b = crops[i];
+    const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
+    if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20))
+      OPB_FAIL(ctx, OPB_ERR_ARG, "whole_body_frame: a crop is wider or taller than 2^20");
+    KpCrop& c = table[i];
+    c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip;
+    c.vh = c.h; c.vw = c.w;
+  }
+  return OPB_OK;
+}
+
+}  // namespace
+
+int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* img, int img_loc, int orig_h,
+                         int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len, const float* inject_paf,
+                         const float* inject_heat, int face_net_size, double face_thresh, int hand_net_size,
+                         double hand_thresh, opb_image_header* header_out, opb_person* persons_out,
+                         opb_wb_part* parts_out, int parts_cap, int* n_parts, double* face_out, int32_t* face_valid,
+                         double* hand_out, int32_t* hand_valid, uint8_t* picture_out) {
+  if (!pose) return OPB_ERR_ARG;
+  // everything is checked before the first enqueue
+  if (!face || !hand) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: a FaceNet and a HandNet context are required");
+  if (pose->kp_out != 0) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the first context must hold the pose net");
+  if (face->kp_out != 71) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the face context does not hold FaceNet");
+  if (hand->kp_out != 22) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the hand context does not hold HandNet");
+  if (pose->precision < 0 || face->precision < 0 || hand->precision < 0)
+    OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: opb_finalize_weights has not been called on every context");
+  if (face->device != pose->device || hand->device != pose->device)
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: the three contexts must be on the same device");
+  if (!img || orig_h <= 0 || orig_w <= 0 || in_h <= 0 || in_w <= 0 || in_h % 8 || in_w % 8 || map_h <= 0 || map_w <= 0)
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: bad frame, input or map size");
+  if (face_net_size <= 0 || face_net_size % 8 || hand_net_size <= 0 || hand_net_size % 8)
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: net sizes must be positive multiples of 8");
+  if (!header_out || !persons_out || !n_parts || parts_cap < 0 ||
+      (parts_cap > 0 && (!parts_out || !face_out || !face_valid || !hand_out || !hand_valid)))
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: bad output arguments");
+  *n_parts = 0;
+  cudaSetDevice(pose->device);
+  const double sx = static_cast<double>(orig_w) / map_w, sy = static_cast<double>(orig_h) / map_h;  // :513-514
+  const int cap = pose->prm.max_persons;
+  const size_t rec_b = sizeof(ImageHeader) + sizeof(PersonOut) * static_cast<size_t>(cap);
+  const WbLayout L = wb_layout(cap);
+  int rc;
+  // (1) one upload of the frame, the device resize and the pipeline of opb_detect_image
+  Chain* ch = nullptr;
+  PostWs* ws = nullptr;
+  if ((rc = get_chain(pose, 1, in_h, in_w, &ch))) return rc;
+  if ((rc = get_post(pose, 1, map_h, map_w, &ws))) return rc;
+  WbOut wo;
+  if ((rc = wb_reserve(pose, cap, 0, rec_b + L.tables_end, &wo))) return rc;
+  const size_t in_b = static_cast<size_t>(orig_h) * orig_w * 3;
+  const uint8_t* d_frame = img;
+  if (img_loc == OPB_HOST) {
+    if ((rc = ensure_ingest(pose, in_b + 512))) return rc;
+    if ((rc = copy_in(pose, pose->ingest_buf, img, in_b, OPB_HOST))) return rc;
+    d_frame = pose->ingest_buf;
+  }
+  if ((rc = launch_resize_u8(pose, d_frame, 1, orig_h, orig_w, ch->img_u8, in_h, in_w))) return rc;
+  ch->img_u8_src = nullptr;
+  // (2) inject_* replace the network output, as in opb_detect_batch
+  if ((rc = run_pipeline(pose, ch, ws, 1, in_h, in_w, map_h, map_w, img_len, inject_paf, inject_heat))) return rc;
+  // (3) the crop boxes, then one download of the records and the tables and one synchronisation
+  if ((rc = wb_launch(pose, ws->headers, ws->persons, cap, sx, sy, wo))) return rc;
+  static_assert(sizeof(ImageHeader) % 16 == 0, "the persons follow the header in the record block");
+  OPB_CUDA(pose, cudaMemcpyAsync(pose->wb_host, ws->headers, rec_b, cudaMemcpyDeviceToHost, pose->stream));
+  OPB_CUDA(pose, cudaMemcpyAsync(pose->wb_host + rec_b, pose->wb_buf, L.tables_end, cudaMemcpyDeviceToHost, pose->stream));
+  OPB_CUDA(pose, cudaStreamSynchronize(pose->stream));
+  const uint8_t* hb = pose->wb_host;
+  std::memcpy(header_out, hb, sizeof(ImageHeader));
+  std::memcpy(persons_out, hb + sizeof(ImageHeader), sizeof(PersonOut) * static_cast<size_t>(cap));
+  const ImageHeader hd = *reinterpret_cast<const ImageHeader*>(hb);
+  if (hd.status != 0) OPB_FAIL(pose, hd.status, "whole_body_frame: the frame's result carries an error status");
+  const WbCounts cnt = *reinterpret_cast<const WbCounts*>(hb + rec_b + L.counts);
+  if (cnt.status != 0) OPB_FAIL(pose, cnt.status, "whole_body_frame: a crop box edge does not fit int32");
+  const WbCrop* h_face = reinterpret_cast<const WbCrop*>(hb + rec_b + L.face);
+  const WbCrop* h_hand = reinterpret_cast<const WbCrop*>(hb + rec_b + L.hand);
+  const WbPart* h_parts = reinterpret_cast<const WbPart*>(hb + rec_b + L.parts);
+  *n_parts = cnt.n_parts;
+  if (cnt.n_parts > parts_cap) OPB_FAIL(pose, OPB_ERR_CAPACITY, "whole_body_frame: more parts than parts_cap");
+  std::vector<KpCrop> ftab, htab;
+  if ((rc = wb_kp_table(pose, h_face, cnt.n_face, ftab))) return rc;
+  if ((rc = wb_kp_table(pose, h_hand, cnt.n_hand, htab))) return rc;
+  for (int i = 0; i < cnt.n_parts; ++i) {
+    const WbPart& p = h_parts[i];
+    const WbCrop& b = p.side == WB_FACE ? h_face[p.row] : h_hand[p.row];
+    parts_out[i] = opb_wb_part{p.side == WB_FACE ? OPB_PART_FACE : OPB_PART_HAND, b.left, b.top, b.right, b.bottom,
+                               p.row, p.person, p.side};
+  }
+  // (4) FaceNet on the face stream and HandNet on the hand stream, both reading the frame in place; both chains are
+  // enqueued before either is collected, so they overlap
+  if (!ftab.empty() && (rc = kp_enqueue_table(face, d_frame, orig_h, orig_w, ftab, face_net_size))) return rc;
+  if (!htab.empty() && (rc = kp_enqueue_table(hand, d_frame, orig_h, orig_w, htab, hand_net_size))) {
+    cudaStreamSynchronize(face->stream);
+    return rc;
+  }
+  int rc_face = OPB_OK, rc_hand = OPB_OK;
+  if (!ftab.empty()) rc_face = kp_peaks_collect(face, face->kp_ws, ftab, face->kp_out - 1, face_thresh, face_out, face_valid);
+  if (!htab.empty()) rc_hand = kp_peaks_collect(hand, hand->kp_ws, htab, hand->kp_out - 1, hand_thresh, hand_out, hand_valid);
+  if (rc_face) { pose->err = face->err; return rc_face; }
+  if (rc_hand) { pose->err = hand->err; return rc_hand; }
+  if (!picture_out) return OPB_OK;
+  // (5) the picture of opb_draw_whole_body, on the resident frame, with the skeleton from the device records
+  const int face_pl = face->kp_out - 1, hand_pl = hand->kp_out - 1;
+  std::vector<int32_t> tab(static_cast<size_t>(cnt.n_parts) * 6);
+  std::vector<int32_t> pts;
+  for (int i = 0; i < cnt.n_parts; ++i) {
+    const opb_wb_part& p = parts_out[i];
+    const bool is_face = p.kind == OPB_PART_FACE;
+    const int count = is_face ? face_pl : hand_pl;
+    const double* o = (is_face ? face_out : hand_out) + static_cast<size_t>(p.row) * count * 3;
+    const int32_t* v = (is_face ? face_valid : hand_valid) + static_cast<size_t>(p.row) * count;
+    const int32_t row[6] = {p.kind, p.left, p.top, p.right, p.bottom, static_cast<int32_t>(pts.size() / 3)};
+    std::copy(row, row + 6, tab.begin() + 6 * i);
+    for (int k = 0; k < count; ++k) {
+      pts.push_back(v[k] ? static_cast<int32_t>(o[3 * k]) : 0);
+      pts.push_back(v[k] ? static_cast<int32_t>(o[3 * k + 1]) : 0);
+      pts.push_back(v[k] ? 1 : 0);
+    }
+  }
+  const int n_points = static_cast<int>(pts.size() / 3);
+  if ((rc = check_parts(pose, reinterpret_cast<const opb_part*>(tab.data()), cnt.n_parts, pts.data(), n_points))) return rc;
+  tab.insert(tab.end(), pts.begin(), pts.end());
+  const int n_poses = hd.n_peaks == 0 ? 0 : hd.n_persons;
+  const size_t px = static_cast<size_t>(orig_h) * orig_w, img_b = (px * 3 + 255) & ~size_t(255);
+  const size_t prio_b = (px * 4 + 255) & ~size_t(255);
+  const size_t poses_b = (static_cast<size_t>(std::max(n_poses, 1)) * OV_JOINTS * 3 * 4 + 255) & ~size_t(255);
+  const size_t tab_b = (tab.size() * 4 + 255) & ~size_t(255);
+  // scratch: [picture | priority plane | int poses | parts and points | flag]
+  if ((rc = ov_reserve(pose, img_b + prio_b + poses_b + tab_b + 256))) return rc;
+  uint8_t* d_out = pose->ov_buf;
+  unsigned int* d_prio = reinterpret_cast<unsigned int*>(pose->ov_buf + img_b);
+  int* d_poses = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b);
+  int* d_tab = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b + poses_b);
+  int* d_bad = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b + poses_b + tab_b);
+  if (!tab.empty() && (rc = copy_in(pose, d_tab, tab.data(), tab.size() * 4, OPB_HOST))) return rc;
+  OPB_CUDA(pose, cudaMemsetAsync(d_prio, 0, px * 4, pose->stream));
+  OPB_CUDA(pose, cudaMemsetAsync(d_bad, 0, 4, pose->stream));
+  const OverlayTables tb = overlay_tables(pose);
+  const OvPart* d_parts = reinterpret_cast<const OvPart*>(d_tab);
+  const int* d_points = d_tab + static_cast<size_t>(cnt.n_parts) * 6;
+  if (n_poses > 0) {
+    const int* base = reinterpret_cast<const int*>(ws->persons);
+    const int stride = static_cast<int>(sizeof(PersonOut) / 4), off_id = 4, off_x = 4 + OPB_N_JOINTS, off_y = 4 + 2 * OPB_N_JOINTS;
+    overlay_poses_from_records_kernel<<<(n_poses * OV_JOINTS + 127) / 128, 128, 0, pose->stream>>>(
+        base + off_x, base + off_y, base + off_id, stride, n_poses, sx, sy, d_poses);
+    pose->launches++;
+  }
+  const long long n_prim = static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) +
+                           static_cast<long long>(cnt.n_parts) * OV_PART_STRIDE;
+  if (n_prim > 0) {
+    overlay_raster_kernel<<<static_cast<unsigned>((n_prim + 63) / 64), 64, 0, pose->stream>>>(
+        d_poses, n_poses, tb, d_prio, orig_h, orig_w, d_bad, d_parts, cnt.n_parts, d_points);
+    pose->launches++;
+  }
+  overlay_paint_kernel<<<static_cast<unsigned>((px + 255) / 256), 256, 0, pose->stream>>>(
+      d_frame, d_prio, static_cast<int>(px), n_poses, tb, d_out, d_parts, 1);
+  pose->launches++;
+  OPB_CUDA(pose, cudaGetLastError());
+  int bad = 0;
+  OPB_CUDA(pose, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, pose->stream));
+  if ((rc = copy_out(pose, picture_out, d_out, px * 3, OPB_HOST))) return rc;
+  OPB_CUDA(pose, cudaStreamSynchronize(pose->stream));
+  if (bad) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: a joint lies outside the image");
+  return OPB_OK;
+}
+
+int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, double sx, double sy, double* unit_out,
+                              int32_t* boxes_out, int32_t* present_out, int32_t* parts_out, int* n_parts) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (n < 0 || n > (1 << 16) || (n > 0 && (!persons || !unit_out || !boxes_out || !present_out || !parts_out)) ||
+      !n_parts || !std::isfinite(sx) || !std::isfinite(sy))
+    OPB_FAIL(ctx, OPB_ERR_ARG, "test_whole_body_boxes: bad arguments");
+  cudaSetDevice(ctx->device);
+  const int cap = std::max(n, 1);
+  const WbLayout L = wb_layout(cap);
+  const size_t rec_b = sizeof(ImageHeader) + sizeof(PersonOut) * static_cast<size_t>(cap);
+  WbOut wo;
+  int rc;
+  if ((rc = wb_reserve(ctx, cap, rec_b, L.total, &wo))) return rc;
+  ImageHeader* d_hd = reinterpret_cast<ImageHeader*>(ctx->wb_buf + L.total);
+  PersonOut* d_persons = reinterpret_cast<PersonOut*>(ctx->wb_buf + L.total + sizeof(ImageHeader));
+  const ImageHeader hd{1, n, 0, 0};
+  if ((rc = copy_in(ctx, d_hd, &hd, sizeof(hd), OPB_HOST))) return rc;
+  if (n > 0 && (rc = copy_in(ctx, d_persons, persons, sizeof(PersonOut) * n, OPB_HOST))) return rc;
+  if ((rc = wb_launch(ctx, d_hd, d_persons, cap, sx, sy, wo))) return rc;
+  OPB_CUDA(ctx, cudaMemcpyAsync(ctx->wb_host, ctx->wb_buf, L.total, cudaMemcpyDeviceToHost, ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  const uint8_t* hb = ctx->wb_host;
+  const WbCounts cnt = *reinterpret_cast<const WbCounts*>(hb + L.counts);
+  if (cnt.status != 0) OPB_FAIL(ctx, cnt.status, "test_whole_body_boxes: a crop box edge does not fit int32");
+  if (n > 0) {
+    std::memcpy(unit_out, hb + L.unit, sizeof(double) * n);
+    std::memcpy(boxes_out, hb + L.box, sizeof(int) * 12 * n);
+    std::memcpy(present_out, hb + L.present, sizeof(int) * n);
+  }
+  const WbPart* parts = reinterpret_cast<const WbPart*>(hb + L.parts);
+  for (int i = 0; i < cnt.n_parts; ++i) {
+    parts_out[2 * i] = parts[i].person;
+    parts_out[2 * i + 1] = parts[i].side;
+  }
+  *n_parts = cnt.n_parts;
   return OPB_OK;
 }
 

@@ -1,7 +1,8 @@
-"""The whole-body result picture of the reference's demo.py (:28-57) in one call.
+"""The whole-body result picture of the reference's demo.py (:28-57) in one call, and the demo's whole frame in one call.
 
     res = draw_whole_body(img, poses, parts)                      # host: the cv2 calls demo.py makes
     res = draw_whole_body(img, poses, parts, engine=det.engine)   # device: the same pixels, one upload, one download
+    poses, scores, parts, owners, res = detect_whole_body(img, pose_detector, face_detector, hand_detector)
 
 `parts` lists (kind, bbox, keypoints) in drawing order -- demo.py's is, person by person, face, left hand, right hand:
 kind "face" (70 keypoints) or "hand" (21), bbox (left, top, right, bottom) as PoseDetector.crop_face / crop_hands
@@ -13,11 +14,13 @@ import numpy as np
 
 try:
     from . import _native
+    from .entity import params
     from .face_detector import draw_face_keypoints
     from .hand_detector import draw_hand_keypoints
     from .pose_detector import draw_person_pose
 except ImportError:  # flat import, like the reference
     import _native
+    from entity import params
     from face_detector import draw_face_keypoints
     from hand_detector import draw_hand_keypoints
     from pose_detector import draw_person_pose
@@ -63,3 +66,58 @@ def draw_whole_body(orig_img, poses, parts, engine=None):
         res = draw(res, kps, (bbox[0], bbox[1]))
         cv2.rectangle(res, (bbox[0], bbox[1]), (bbox[2], bbox[3]), (255, 255, 255), 1)
     return res
+
+
+_SIDES = {_native.SIDE_FACE: "face", _native.SIDE_LEFT: "left", _native.SIDE_RIGHT: "right"}
+
+
+def detect_whole_body(img, pose_detector, face_detector, hand_detector, draw=True):
+    """demo.py's frame (:24-57) in one device call (opb_whole_body_frame): the pose pass, every person's crop_face and
+    crop_hands boxes, FaceNet and HandNet on all crops (concurrently, on the face and the hand detector's contexts), and
+    the result picture.  Returns (poses, scores, parts, owners, picture):
+      poses, scores  exactly pose_detector(img).  The demo's own array ends with its hand joints moved by crop_hands'
+                     in-place `+=`; that side effect is not reproduced.
+      parts          the (kind, bbox, keypoints) list draw_whole_body takes, in the demo's order (per person: face,
+                     left hand, right hand), bbox as Python ints, keypoints as the detectors return them.
+      owners         (person index, "face" | "left" | "right") per part.
+      picture        draw_whole_body(img, poses, parts), or None with draw=False.
+    Unlike the demo, which raises on them, a person whose unit length is not finite (no limb of positive length) gets
+    no part and a box of zero width or height is no part.  ValueError for a precise PoseDetector, detectors on
+    different devices, or a face / hand detector in the wrong slot; a result status error raises as __call__ does.
+    Afterwards pose_detector.draw_last_result(img) draws this frame's skeleton."""
+    return _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw)
+
+
+def _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw, inject_paf=None, inject_heat=None):
+    """detect_whole_body with inject_paf / inject_heat: device maps [1,38,H/8,W/8] / [1,19,H/8,W/8] that replace the
+    pose network's output, as in Engine.detect_batch (stick-figure persons for tests and benchmarks)"""
+    if getattr(pose_detector, "precise", False):
+        raise ValueError("detect_whole_body runs the single-scale path; a precise PoseDetector is not supported")
+    pe, fe, he = pose_detector.engine, face_detector.engine, hand_detector.engine
+    if getattr(pe, "kp_channels", 0) != 0:
+        raise ValueError("pose_detector must hold CocoPoseNet")
+    if getattr(fe, "kp_channels", 0) != 71:
+        raise ValueError("face_detector must hold FaceNet (71 output channels), got %d" % getattr(fe, "kp_channels", 0))
+    if getattr(he, "kp_channels", 0) != 22:
+        raise ValueError("hand_detector must hold HandNet (22 output channels), got %d" % getattr(he, "kp_channels", 0))
+    if not pe.device == fe.device == he.device:
+        raise ValueError("the detectors are on different devices (%d, %d, %d)" % (pe.device, fe.device, he.device))
+    img = np.asarray(img)
+    if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+        raise ValueError("img must be a uint8 [H, W, 3] BGR frame, got %s %s" % (img.dtype, img.shape))
+    oh, ow = img.shape[:2]
+    in_w, in_h = pose_detector.compute_optimal_size(img, params['inference_img_size'])
+    map_w, map_h = pose_detector.compute_optimal_size(img, params['heatmap_size'])
+    headers, persons, table, faces, hands, picture = pe.whole_body_frame(
+        fe, he, img, in_h, in_w, map_h, map_w, map_w, params["face_inference_img_size"],
+        params['face_heatmap_peak_thresh'], params["hand_inference_img_size"], params['hand_heatmap_peak_thresh'],
+        draw=draw, inject_paf=inject_paf, inject_heat=inject_heat)
+    pose_detector._last_scale = (ow / map_w, oh / map_h)
+    poses, scores = pose_detector._poses_from_records(headers[0], persons[0], ow / map_w, oh / map_h)
+    parts, owners = [], []
+    for r in table:
+        face = int(r["kind"]) == _native.PART_FACE
+        kps = (faces if face else hands)[int(r["row"])]
+        parts.append(("face" if face else "hand", (int(r["left"]), int(r["top"]), int(r["right"]), int(r["bottom"])), kps))
+        owners.append((int(r["person"]), _SIDES[int(r["side"])]))
+    return poses, scores, parts, owners, picture

@@ -331,6 +331,54 @@ int opb_test_cascade_windows(opb_ctx* ctx, const uint8_t* img, int img_loc, int 
                              double scale_factor, int min_w, int min_h, int max_w, int max_h, int32_t* codes_out,
                              double* sums_out, int cap, int* n_out);
 
+/* ---- the whole-body frame of demo.py:24-57 in one call ----
+ * opb_whole_body_frame: pose (CocoPoseNet), face (FaceNet) and hand (HandNet) are three contexts on one device.  In order:
+ *   1. one upload of the BGR frame [orig_h, orig_w, 3] to the pose context (none with OPB_DEVICE: read in place), the
+ *      device resize to (in_h, in_w) and the pipeline of opb_detect_image; inject_paf / inject_heat as in
+ *      opb_detect_batch (device maps that replace the network output, or NULL);
+ *   2. the crop-box kernel (csrc/whole_body.cuh) on the device records: per person PoseDetector.get_unit_length,
+ *      crop_face and crop_hands of pose_detector.py in float64, bit for bit, with sx = orig_w / map_w and
+ *      sy = orig_h / map_h; then one download of the records and the box tables and one synchronisation;
+ *   3. FaceNet on the face crops on the face context's stream and HandNet on the hand crops (left hands mirrored) on the
+ *      hand context's stream, both reading the frame in place from the pose context's buffer; both are enqueued before
+ *      either is collected, so they overlap.  Each equals opb_keypoints_detect_crops on the same boxes; a net without
+ *      crops is skipped;
+ *   4. with picture_out != NULL, the picture of opb_draw_whole_body on the resident frame -- the skeleton from the
+ *      device records (as opb_draw_last_result), then the parts -- and one download of it.
+ * Deviation from demo.py, which raises on such persons: a person whose unit length is not finite (no limb of positive
+ * length) gets no part, and a box of non-positive width or height is not a part.  Parts come in the demo's order (per
+ * person: face, left hand, right hand).  Outputs: header_out and persons_out (max_persons records) as
+ * opb_detect_image; parts_out [parts_cap], *n_parts; face_out [parts_cap][70][3] / face_valid [parts_cap][70] and
+ * hand_out [parts_cap][21][3] / hand_valid [parts_cap][21] as opb_keypoints_detect_crops, row p.row for part p;
+ * picture_out [orig_h, orig_w, 3] host.  What crosses contexts: the frame buffer of the pose context, read by the face
+ * and hand streams after the pose stream was synchronised.  No context has work pending on a successful return, and the
+ * pose context holds this frame's result (opb_draw_last_result, opb_get_image_detail).
+ * OPB_ERR_ARG / OPB_ERR_STATE before anything is enqueued for contexts on different devices, a context that does not
+ * hold its net or has no finalised weights, and bad sizes or outputs; the frame's record status (as opb_detect_batch
+ * reports it in the header) is returned as the error; OPB_ERR_UNSUPPORTED for a box edge beyond int32;
+ * OPB_ERR_CAPACITY when the parts do not fit parts_cap (*n_parts holds the count). */
+enum { OPB_SIDE_FACE = 0, OPB_SIDE_LEFT = 1, OPB_SIDE_RIGHT = 2 };
+typedef struct opb_wb_part {
+  int32_t kind;                       /* OPB_PART_FACE or OPB_PART_HAND                                          */
+  int32_t left, top, right, bottom;   /* the crop box of crop_face / crop_hands                                 */
+  int32_t row;                        /* the part's keypoint row in face_out / hand_out                         */
+  int32_t person;                     /* index of the person in persons_out                                     */
+  int32_t side;                       /* OPB_SIDE_FACE / OPB_SIDE_LEFT / OPB_SIDE_RIGHT                        */
+} opb_wb_part;
+int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* img, int img_loc, int orig_h,
+                         int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len, const float* inject_paf,
+                         const float* inject_heat, int face_net_size, double face_thresh, int hand_net_size,
+                         double hand_thresh, opb_image_header* header_out, opb_person* persons_out,
+                         opb_wb_part* parts_out, int parts_cap, int* n_parts, double* face_out, int32_t* face_valid,
+                         double* hand_out, int32_t* hand_valid, uint8_t* picture_out);
+/* Test hook: the crop-box kernel of opb_whole_body_frame on n host person records (all persons of one image).
+ *   unit_out [n] float64 unit lengths (NaN without a positive limb), boxes_out [n][3][4] (face, left hand, right hand:
+ *   left, top, right, bottom), present_out [n] (bit k: box k exists -- its joint is present and the unit length is
+ *   finite -- boxes without the bit are not written), parts_out [3n][2] (person, side) of the kept parts in order,
+ *   *n_parts.  OPB_ERR_UNSUPPORTED when a box edge does not fit int32. */
+int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, double sx, double sy, double* unit_out,
+                              int32_t* boxes_out, int32_t* present_out, int32_t* parts_out, int* n_parts);
+
 /* device pointers of the last opb_detect_batch outputs/intermediates (valid until the next
  * call with a different shape): 0 paf_lo, 1 heat_lo, 2 pafs (full-res), 3 heatmaps (full-res),
  * 4 headers, 5 persons, 6 peak table ([N,max_peaks] of {int32 type,x,y; float score})       */
