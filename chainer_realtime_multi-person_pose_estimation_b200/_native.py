@@ -42,6 +42,13 @@ SIDE_FACE, SIDE_LEFT, SIDE_RIGHT = 0, 1, 2
 PART_POINTS = {PART_FACE: 70, PART_HAND: 21}
 assert PERSON_DTYPE.itemsize == 240 and HEADER_DTYPE.itemsize == 16 and CROP_DTYPE.itemsize == 24
 assert PART_DTYPE.itemsize == 24 and WB_PART_DTYPE.itemsize == 32
+CONV_PROBLEM_DTYPE = np.dtype([(f, "<i4") for f in (
+    "in_h", "in_w", "in_c", "in_ctot", "in_coff", "out_h", "out_w", "out_c", "out_ctot", "out_coff", "cout_valid", "relu",
+    "pool", "has_out32", "cin_pad", "cout_pad")] + [("acc_scale", "<f4"), ("reserved", "<i4")])    # opb_conv_problem
+CONV_RECORD_DTYPE = np.dtype([("tag", "S32"), ("wkey", "S48", (2,))] + [(f, "<i4") for f in (
+    "ks", "bn", "drain", "comp", "n_problems", "grid", "shared_in", "reserved")] + [
+    ("prob", CONV_PROBLEM_DTYPE, (2,))])                                                              # opb_conv_record
+assert CONV_PROBLEM_DTYPE.itemsize == 72 and CONV_RECORD_DTYPE.itemsize == 304
 
 
 def crop_table(bboxes, flips=None):
@@ -139,6 +146,9 @@ _SIGNATURES = {
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "opb_test_conv_first": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "opb_test_chain_convs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
+    "opb_test_chain_conv_run": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "opb_cascade_load": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "opb_cascade_detect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
@@ -774,3 +784,22 @@ class Engine(object):
         self._check(self.lib.opb_test_conv_first(self.ctx, _ptr(x), int(is_u8), n, h, w, float(u8_denom), _ptr(W),
                                                  _ptr(b), int(precision), _ptr(out)))
         return out
+
+    def test_chain_convs(self, n, h, w):
+        """The conv launches of the loaded model's chain at (n, h, w): a CONV_RECORD_DTYPE array in launch order."""
+        count = C.c_int(0)
+        rc = self.lib.opb_test_chain_convs(self.ctx, int(n), int(h), int(w), None, 0, C.byref(count))
+        if rc not in (0, ERR_CAPACITY):
+            self._check(rc)
+        recs = np.zeros(count.value, CONV_RECORD_DTYPE)
+        self._check(self.lib.opb_test_chain_convs(self.ctx, int(n), int(h), int(w), _ptr(recs), len(recs), C.byref(count)))
+        return recs
+
+    def test_chain_conv_run(self, n, h, w, index, in0, in1, out_io, out32=(None, None)):
+        """Runs conv launch `index` of that chain alone.  in0 / in1: raw input tensors (uint8 arrays of the whole
+        tensor; in1 only when problem 1 reads another tensor); out_io (uint8, whole output tensor) and the float32 maps
+        of out32 are uploaded as prior content and overwritten in place with what the launch left there."""
+        arrs = [in0, in1, out_io] + list(out32)
+        for a in arrs:
+            assert a is None or (isinstance(a, np.ndarray) and a.flags.c_contiguous)
+        self._check(self.lib.opb_test_chain_conv_run(self.ctx, int(n), int(h), int(w), int(index), *map(_ptr, arrs)))

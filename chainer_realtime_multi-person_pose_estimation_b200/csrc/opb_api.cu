@@ -72,6 +72,13 @@ struct Act {              // NHWC fp16 activation tensor, channels [hi C | lo C]
 
 enum OpKind { OP_FIRST, OP_CONV, OP_POOL };
 
+struct ConvRec {          // what one problem of a conv op was built from (read back by the test hooks only)
+  Act in, out;
+  int in_coff = 0, out_coff = 0, cout_valid = 0, relu = 0, pool = 0;
+  float* out32 = nullptr;
+  std::string wkey;
+};
+
 struct Op {
   OpKind kind;
   std::string tag;
@@ -81,6 +88,7 @@ struct Op {
   CUtensorMap tmA[2], tmB[2];
   ConvParams P;
   int grid = 0;
+  ConvRec rec[2];
   // OP_FIRST / OP_POOL
   const __half* in = nullptr;
   __half* out = nullptr;
@@ -553,6 +561,16 @@ int add_conv(opb_ctx* ctx, Chain* ch, const std::string& tag, const ConvSpec& s)
     pr.relu = s.relu;
     pr.pool = s.pool;
     pr.acc_scale = w.acc_scale;
+    ConvRec& rec = op.rec[p];
+    rec.in = *s.in[p];
+    if (s.out[p]) rec.out = *s.out[p];
+    rec.in_coff = s.in_coff[p];
+    rec.out_coff = s.out_coff[p];
+    rec.cout_valid = s.cout_valid[p];
+    rec.relu = s.relu;
+    rec.pool = s.pool;
+    rec.out32 = s.out32[p];
+    rec.wkey = s.wkey[p];
   }
   if (s.n_problems == 1) { op.tmA[1] = op.tmA[0]; op.tmB[1] = op.tmB[0]; P.prob[1] = P.prob[0]; }
   const int total_tiles = P.n_problems * P.n_blocks * P.N * P.tiles_y * P.tiles_x;
@@ -3481,6 +3499,88 @@ int opb_test_conv_first(opb_ctx* ctx, const void* x, int x_is_u8, int n, int h, 
   ctx->b_first = saved_b;
   ctx->u8_denom = saved_denom;
   return rc;
+}
+
+static_assert(sizeof(opb_conv_problem) == 72, "opb_conv_problem size");
+static_assert(sizeof(opb_conv_record) == 32 + 96 + 32 + 2 * 72, "opb_conv_record size");
+
+static void copy_name(char* dst, size_t cap, const std::string& s) {
+  std::memset(dst, 0, cap);
+  std::memcpy(dst, s.data(), std::min(s.size(), cap - 1));
+}
+
+int opb_test_chain_convs(opb_ctx* ctx, int n, int h, int w, opb_conv_record* out, int cap, int* count) {
+  if (!ctx || !count || cap < 0 || (cap && !out)) return OPB_ERR_ARG;
+  cudaSetDevice(ctx->device);
+  Chain* ch = nullptr;
+  int rc = get_chain(ctx, n, h, w, &ch);
+  if (rc) return rc;
+  int k = 0;
+  for (const Op& op : ch->ops) {
+    if (op.kind != OP_CONV) continue;
+    if (k < cap) {
+      opb_conv_record& r = out[k];
+      std::memset(&r, 0, sizeof(r));
+      copy_name(r.tag, sizeof(r.tag), op.tag);
+      r.ks = op.ks; r.bn = op.bn; r.drain = op.drain; r.comp = op.P.comp; r.n_problems = op.P.n_problems;
+      r.grid = op.grid;
+      r.shared_in = op.P.n_problems == 2 && op.rec[0].in.p == op.rec[1].in.p;
+      for (int p = 0; p < op.P.n_problems; ++p) {
+        const ConvRec& c = op.rec[p];
+        const PackedW& pw = ctx->packed.at(c.wkey);
+        copy_name(r.wkey[p], sizeof(r.wkey[p]), c.wkey);
+        opb_conv_problem& q = r.prob[p];
+        q.in_h = c.in.H; q.in_w = c.in.W; q.in_c = c.in.C; q.in_ctot = c.in.Ctot; q.in_coff = c.in_coff;
+        q.out_h = c.out.H; q.out_w = c.out.W; q.out_c = c.out.C; q.out_ctot = c.out.Ctot; q.out_coff = c.out_coff;
+        q.cout_valid = c.cout_valid; q.relu = c.relu; q.pool = c.pool; q.has_out32 = c.out32 != nullptr;
+        q.cin_pad = pw.cin_pad; q.cout_pad = pw.cout_pad; q.acc_scale = pw.acc_scale;
+      }
+    }
+    ++k;
+  }
+  *count = k;
+  if (k > cap) OPB_FAIL(ctx, OPB_ERR_CAPACITY, "test chain convs: " + std::to_string(k) + " records, capacity " + std::to_string(cap));
+  return OPB_OK;
+}
+
+int opb_test_chain_conv_run(opb_ctx* ctx, int n, int h, int w, int index, const void* in0, const void* in1,
+                            void* out_io, float* out32_0, float* out32_1) {
+  if (!ctx || !in0 || !out_io) return OPB_ERR_ARG;
+  cudaSetDevice(ctx->device);
+  Chain* ch = nullptr;
+  int rc = get_chain(ctx, n, h, w, &ch);
+  if (rc) return rc;
+  const Op* op = nullptr;
+  int k = 0;
+  for (const Op& o : ch->ops) {
+    if (o.kind != OP_CONV) continue;
+    if (k++ == index) { op = &o; break; }
+  }
+  if (!op) OPB_FAIL(ctx, OPB_ERR_ARG, "test chain conv run: no conv launch " + std::to_string(index));
+  const int np = op->P.n_problems;
+  const ConvRec* rec = op->rec;
+  const Act& out = rec[0].out;
+  if (!out.p) OPB_FAIL(ctx, OPB_ERR_UNSUPPORTED, "test chain conv run: the op writes no activation tensor");
+  float* const o32[2] = {out32_0, out32_1};
+  for (int p = 0; p < np; ++p) {
+    if (rec[p].out.p != out.p) OPB_FAIL(ctx, OPB_ERR_UNSUPPORTED, "test chain conv run: the problems write two tensors");
+    if (rec[p].in.p == out.p) OPB_FAIL(ctx, OPB_ERR_UNSUPPORTED, "test chain conv run: the op reads its own output");
+    if (rec[p].out32 && !o32[p]) OPB_FAIL(ctx, OPB_ERR_ARG, "test chain conv run: missing fp32 map buffer");
+  }
+  const bool second_in = np == 2 && rec[1].in.p != rec[0].in.p;
+  if (second_in && !in1) OPB_FAIL(ctx, OPB_ERR_ARG, "test chain conv run: problem 1 reads its own input tensor");
+  auto planes_bytes = [&](int p) { return static_cast<size_t>(out.N) * rec[p].cout_valid * out.H * out.W * sizeof(float); };
+  OPB_CUDA(ctx, cudaMemcpyAsync(rec[0].in.p, in0, rec[0].in.bytes(), cudaMemcpyHostToDevice, ctx->stream));
+  if (second_in) OPB_CUDA(ctx, cudaMemcpyAsync(rec[1].in.p, in1, rec[1].in.bytes(), cudaMemcpyHostToDevice, ctx->stream));
+  OPB_CUDA(ctx, cudaMemcpyAsync(out.p, out_io, out.bytes(), cudaMemcpyHostToDevice, ctx->stream));
+  for (int p = 0; p < np; ++p)
+    if (rec[p].out32) OPB_CUDA(ctx, cudaMemcpyAsync(rec[p].out32, o32[p], planes_bytes(p), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = launch_op(ctx, ch, *op))) return rc;
+  OPB_CUDA(ctx, cudaMemcpyAsync(out_io, out.p, out.bytes(), cudaMemcpyDeviceToHost, ctx->stream));
+  for (int p = 0; p < np; ++p)
+    if (rec[p].out32) OPB_CUDA(ctx, cudaMemcpyAsync(o32[p], rec[p].out32, planes_bytes(p), cudaMemcpyDeviceToHost, ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return OPB_OK;
 }
 
 }  // extern "C"

@@ -440,6 +440,36 @@ int opb_test_conv(opb_ctx* ctx, const float* x, int n, int h, int w, int cin, co
 int opb_test_conv_first(opb_ctx* ctx, const void* x, int x_is_u8, int n, int h, int w, float u8_denom,
                         const float* W, const float* b, int precision_mode, uint8_t* out);
 
+/* One problem of a conv launch of a chain: its input and output activation tensors (NHWC, `c` channels per plane,
+ * `ctot` = c (fast) or 2c (parity: [hi | lo] fp16; compensated: [hi fp16 | 2c correction bytes]) halves per pixel), the
+ * channel offsets it reads and writes, and the packed weights it multiplies.                                        */
+typedef struct opb_conv_problem {
+  int32_t in_h, in_w, in_c, in_ctot, in_coff;
+  int32_t out_h, out_w, out_c, out_ctot, out_coff;   /* out_h, out_w: after the fused max-pool, if any         */
+  int32_t cout_valid, relu, pool, has_out32;         /* has_out32: also writes fp32 maps [N][cout_valid][h][w] */
+  int32_t cin_pad, cout_pad;
+  float acc_scale;
+  int32_t reserved;
+} opb_conv_problem;
+typedef struct opb_conv_record {
+  char tag[32];
+  char wkey[2][48];                                  /* packed-weight key per problem                          */
+  int32_t ks, bn, drain, comp, n_problems, grid;
+  int32_t shared_in;                                 /* the problems read one tensor (at their own offsets)    */
+  int32_t reserved;
+  opb_conv_problem prob[2];
+} opb_conv_record;
+/* The conv launches of the loaded model's chain at (n, h, w) (built if needed), one record per launch in launch
+ * order.  *count = number of launches; OPB_ERR_CAPACITY when it exceeds cap (the first cap records are written). */
+int opb_test_chain_convs(opb_ctx* ctx, int n, int h, int w, opb_conv_record* out, int cap, int* count);
+/* Runs conv launch `index` of that chain on its own: uploads the raw bytes of each problem's whole input tensor (in0;
+ * in1 when problem 1 reads another tensor), out_io as the prior content of the whole output tensor and out32_p as the
+ * prior content of problem p's fp32 maps (when it has them), launches the op, and downloads all of them back into
+ * out_io / out32_p.  The chain's activations are scratch for this hook.  OPB_ERR_ARG for a bad index or a missing
+ * buffer; OPB_ERR_UNSUPPORTED for an op that reads its own output tensor or whose problems write two tensors.     */
+int opb_test_chain_conv_run(opb_ctx* ctx, int n, int h, int w, int index, const void* in0, const void* in1,
+                            void* out_io, float* out32_0, float* out32_1);
+
 #ifdef __cplusplus
 }
 #endif
