@@ -165,6 +165,14 @@ _SIGNATURES = {
                                        C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "opb_test_whole_body_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
+    "opb_whole_body_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.c_double, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
+    "opb_test_whole_body_boxes_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double,
+                                                  C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -716,6 +724,68 @@ class Engine(object):
         faces = [self._keypoint_list(o, v) for o, v in zip(face_out[:n_face], face_valid[:n_face])]
         hands = [self._keypoint_list(o, v) for o, v in zip(hand_out[:n.value - n_face], hand_valid[:n.value - n_face])]
         return headers, persons, parts, faces, hands, picture
+
+    def whole_body_batch(self, face_engine, hand_engine, frames, in_h, in_w, map_h, map_w, img_len, face_net_size,
+                         face_thresh, hand_net_size, hand_thresh, draw=True, inject_paf=None, inject_heat=None):
+        """opb_whole_body_batch on N equally sized frames [N,H,W,3] uint8: returns (headers[N], persons[N, max_persons],
+        parts (WB_PART_DTYPE [k]), frame_parts int [N + 1], face keypoint lists by row, hand keypoint lists by row,
+        pictures [N,H,W,3] uint8 or None).  A frame's record status raises what raise_for_status raises for it.
+        inject_*: device pointers (ints) to [N,38|19,in_h/8,in_w/8] maps, or None."""
+        frames = np.ascontiguousarray(frames, np.uint8)
+        n, oh, ow, _ = frames.shape
+        headers = np.zeros(n, HEADER_DTYPE)
+        persons = np.empty((n, self.max_persons), PERSON_DTYPE)
+        cap = 3 * self.max_persons * n                 # every person has at most a face and two hands
+        parts = np.empty(cap, WB_PART_DTYPE)
+        frame_parts = np.zeros(n + 1, np.int32)
+        fpl = max(getattr(face_engine, "kp_channels", 0) - 1, 0)
+        hpl = max(getattr(hand_engine, "kp_channels", 0) - 1, 0)
+        face_out, face_valid = np.empty((cap, fpl, 3), np.float64), np.empty((cap, fpl), np.int32)
+        hand_out, hand_valid = np.empty((cap, hpl, 3), np.float64), np.empty((cap, hpl), np.int32)
+        pictures = np.empty_like(frames) if draw else None
+        k = C.c_int(0)
+        rc = self.lib.opb_whole_body_batch(
+            self.ctx, face_engine.ctx, hand_engine.ctx, _ptr(frames), OPB_HOST, n, oh, ow, in_h, in_w, map_h, map_w,
+            float(img_len), C.c_void_p(int(inject_paf)) if inject_paf else None,
+            C.c_void_p(int(inject_heat)) if inject_heat else None, int(face_net_size), float(face_thresh),
+            int(hand_net_size), float(hand_thresh), _ptr(headers), _ptr(persons), _ptr(parts), cap, C.byref(k),
+            _ptr(frame_parts), _ptr(face_out), _ptr(face_valid), _ptr(hand_out), _ptr(hand_valid), _ptr(pictures))
+        if rc != 0:
+            bad = np.flatnonzero(headers["status"] != 0)
+            if len(bad) and int(headers["status"][bad[0]]) == rc:   # a frame's record status, as detect_batch raises it
+                self.raise_for_status(rc)
+            self._check(rc)
+        parts = parts[:k.value].copy()
+        n_face = int((parts["kind"] == PART_FACE).sum())
+        faces = [self._keypoint_list(o, v) for o, v in zip(face_out[:n_face], face_valid[:n_face])]
+        hands = [self._keypoint_list(o, v) for o, v in zip(hand_out[:k.value - n_face], hand_valid[:k.value - n_face])]
+        return headers, persons, parts, frame_parts, faces, hands, pictures
+
+    def test_whole_body_boxes_batch(self, headers, persons, sx, sy):
+        """Test hook: the crop-box kernel on the host records of N frames, headers (HEADER_DTYPE [N]) and persons
+        (PERSON_DTYPE [N, cap]), in one launch -> per frame a dict with status, unit [cap], boxes [cap,3,4],
+        present [cap], face / hand (CROP_DTYPE, the frame's compacted tables) and parts int32 [k, 3] (person, side,
+        row)."""
+        hd = np.ascontiguousarray(headers, HEADER_DTYPE)
+        rec = np.ascontiguousarray(persons, PERSON_DTYPE)
+        n, cap = rec.shape
+        assert len(hd) == n
+        counts = np.empty((n, 4), np.int32)
+        unit = np.empty((n, cap), np.float64)
+        boxes = np.empty((n, cap, 3, 4), np.int32)
+        present = np.empty((n, cap), np.int32)
+        face = np.empty((n, cap), CROP_DTYPE)
+        hand = np.empty((n, 2 * cap), CROP_DTYPE)
+        parts = np.empty((n, 3 * cap, 4), np.int32)
+        self._check(self.lib.opb_test_whole_body_boxes_batch(self.ctx, _ptr(hd), _ptr(rec), n, cap, float(sx), float(sy),
+                                                             _ptr(counts), _ptr(unit), _ptr(boxes), _ptr(present),
+                                                             _ptr(face), _ptr(hand), _ptr(parts)))
+        out = []
+        for f in range(n):
+            status, nf, nh, k = (int(v) for v in counts[f])
+            out.append(dict(status=status, unit=unit[f], boxes=boxes[f], present=present[f], face=face[f, :nf].copy(),
+                            hand=hand[f, :nh].copy(), parts=parts[f, :k][:, [1, 0, 2]].copy()))
+        return out
 
     def test_whole_body_boxes(self, persons, sx, sy):
         """Test hook: the crop-box kernel on host person records (PERSON_DTYPE [n]) -> (unit lengths float64 [n],

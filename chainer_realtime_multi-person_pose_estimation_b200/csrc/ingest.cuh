@@ -72,6 +72,7 @@ struct KpCrop {
   int flip;             // canvas mirrored before the net; peak positions reported in the unmirrored canvas
   int tile0;            // first 32x8 tile of the crop in the ragged tile enumeration
   int vh, vw;           // valid extent of the canvas (unmirrored): pixels with y >= vh or x >= vw are zero
+  int frame;            // the crop's frame in a batch of equally sized frames (0 for a single frame)
   double sx, sy;        // cv2.resize scales canvas -> net: 1 / (net / w), 1 / (net / h)
 };
 
@@ -95,16 +96,18 @@ struct CropCanvasU8 {       // crop_image(frame, bbox) (+ flip) read in place
   }
 };
 
-// cv2.resize(flip?(crop_image(frame, crop)), (net, net)) of crops[0..n_real) into dst [gridDim.z][net][net][3]; the
-// slots n_real..gridDim.z-1 (padding of a fixed-size chunk) are zeroed.  grid (ceil(net/32), ceil(net/8), slots)
+// cv2.resize(flip?(crop_image(frames[crop.frame], crop)), (net, net)) of crops[0..n_real) into
+// dst [gridDim.z][net][net][3]; frames [*][fh][fw][3]; the slots n_real..gridDim.z-1 (padding of a fixed-size chunk)
+// are zeroed.  grid (ceil(net/32), ceil(net/8), slots)
 __global__ void __launch_bounds__(256)
-crop_resize_linear_u8_kernel(const uint8_t* __restrict__ frame, int fh, int fw, const KpCrop* __restrict__ crops,
+crop_resize_linear_u8_kernel(const uint8_t* __restrict__ frames, int fh, int fw, const KpCrop* __restrict__ crops,
                              int n_real, uint8_t* __restrict__ dst, int net) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, n = blockIdx.z;
   if (x >= net || y >= net) return;
   uint8_t* o = dst + ((static_cast<size_t>(n) * net + y) * net + x) * 3;
   if (n >= n_real) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
   const KpCrop k = crops[n];
+  const uint8_t* frame = frames + static_cast<size_t>(k.frame) * fh * fw * 3;
   const CropCanvasU8 s{frame, fh, fw, k.top, k.left, k.w, k.flip, k.vh, k.vw};
   cv_linear_pixel(s, k.h, k.w, x, y, k.sx, k.sy, o);
 }

@@ -3028,18 +3028,19 @@ int opb_test_cascade_windows(opb_ctx* ctx, const uint8_t* img, int img_loc, int 
 // ---------------------------------------------------------------- the whole-body frame of demo.py (csrc/whole_body.cuh)
 namespace {
 
-// Device block of the box kernel's outputs for `cap` persons, in the order the frame call downloads it: the counts and
-// the three compacted tables first, then the per-person unit lengths, boxes and present bits (test hook only).
+// Device block of the box kernel's outputs for `n` frames of `cap` persons, in the order the frame call downloads it:
+// the counts and the three compacted tables first, then the per-person unit lengths, boxes and present bits (test
+// hooks only).  Frame f's section of each array starts at f * cap persons (whole_body_boxes_kernel).
 struct WbLayout {
   size_t counts, face, hand, parts, tables_end, unit, box, present, total;
 };
 
-WbLayout wb_layout(int cap) {
+WbLayout wb_layout(int cap, int n = 1) {
   auto al = [](size_t v) { return (v + 255) & ~size_t(255); };
-  const size_t c = static_cast<size_t>(cap);
+  const size_t c = static_cast<size_t>(cap) * n;
   WbLayout L;
   L.counts = 0;
-  L.face = al(sizeof(WbCounts));
+  L.face = al(sizeof(WbCounts) * n);
   L.hand = L.face + al(sizeof(WbCrop) * c);
   L.parts = L.hand + al(sizeof(WbCrop) * 2 * c);
   L.tables_end = L.parts + al(sizeof(WbPart) * 3 * c);
@@ -3050,10 +3051,10 @@ WbLayout wb_layout(int cap) {
   return L;
 }
 
-// Grows ctx->wb_buf to the layout of `cap` persons plus `extra` bytes after it, and the pinned ctx->wb_host to
-// `host_bytes`.
-int wb_reserve(opb_ctx* ctx, int cap, size_t extra, size_t host_bytes, WbOut* out) {
-  const WbLayout L = wb_layout(cap);
+// Grows ctx->wb_buf to the layout of `n` frames of `cap` persons plus `extra` bytes after it, and the pinned
+// ctx->wb_host to `host_bytes`.
+int wb_reserve(opb_ctx* ctx, int cap, int n, size_t extra, size_t host_bytes, WbOut* out) {
+  const WbLayout L = wb_layout(cap, n);
   if (ctx->wb_bytes < L.total + extra) {
     if (ctx->wb_buf) { OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->wb_buf); ctx->wb_buf = nullptr; }
     ctx->wb_bytes = 0;
@@ -3077,131 +3078,212 @@ int wb_reserve(opb_ctx* ctx, int cap, size_t extra, size_t host_bytes, WbOut* ou
   return OPB_OK;
 }
 
-int wb_launch(opb_ctx* ctx, const ImageHeader* d_hd, const PersonOut* d_persons, int cap, double sx, double sy,
+// Ragged-map budget per net of one group of frames in opb_whole_body_batch: 2^30 floats, i.e. 4 GiB for each of the
+// two map buffers
+constexpr size_t kWbGroupFloats = size_t(1) << 30;
+
+// One launch for n frames: headers d_hd[n], persons d_persons[n][cap]
+int wb_launch(opb_ctx* ctx, const ImageHeader* d_hd, const PersonOut* d_persons, int n, int cap, double sx, double sy,
               const WbOut& out) {
-  whole_body_boxes_kernel<<<1, WB_THREADS, 0, ctx->stream>>>(d_hd, d_persons, cap, sx, sy, out);
+  whole_body_boxes_kernel<<<n, WB_THREADS, 0, ctx->stream>>>(d_hd, d_persons, cap, sx, sy, out);
   ctx->launches++;
   OPB_CUDA(ctx, cudaGetLastError());
   return OPB_OK;
 }
 
-// opb_crop rows -> the KpCrop table of opb_keypoints_detect_crops
-int wb_kp_table(opb_ctx* ctx, const WbCrop* crops, int n, std::vector<KpCrop>& table) {
-  table.assign(n, KpCrop{});
+// opb_crop rows of frame `frame` -> KpCrop rows appended to the table of opb_keypoints_detect_crops
+int wb_kp_table(opb_ctx* ctx, const WbCrop* crops, int n, int frame, std::vector<KpCrop>& table) {
   for (int i = 0; i < n; ++i) {
     const WbCrop& b = crops[i];
     const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
     if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20))
-      OPB_FAIL(ctx, OPB_ERR_ARG, "whole_body_frame: a crop is wider or taller than 2^20");
-    KpCrop& c = table[i];
+      OPB_FAIL(ctx, OPB_ERR_ARG, "whole_body_batch: a crop is wider or taller than 2^20");
+    KpCrop c{};
     c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip;
-    c.vh = c.h; c.vw = c.w;
+    c.vh = c.h; c.vw = c.w; c.frame = frame;
+    table.push_back(c);
   }
   return OPB_OK;
 }
 
 }  // namespace
 
-int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* img, int img_loc, int orig_h,
-                         int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len, const float* inject_paf,
-                         const float* inject_heat, int face_net_size, double face_thresh, int hand_net_size,
-                         double hand_thresh, opb_image_header* header_out, opb_person* persons_out,
-                         opb_wb_part* parts_out, int parts_cap, int* n_parts, double* face_out, int32_t* face_valid,
-                         double* hand_out, int32_t* hand_valid, uint8_t* picture_out) {
+int opb_whole_body_batch(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* frames, int frames_loc, int n,
+                         int orig_h, int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len,
+                         const float* inject_paf, const float* inject_heat, int face_net_size, double face_thresh,
+                         int hand_net_size, double hand_thresh, opb_image_header* headers_out, opb_person* persons_out,
+                         opb_wb_part* parts_out, int parts_cap, int* n_parts, int* frame_parts, double* face_out,
+                         int32_t* face_valid, double* hand_out, int32_t* hand_valid, uint8_t* pictures_out) {
   if (!pose) return OPB_ERR_ARG;
   // everything is checked before the first enqueue
-  if (!face || !hand) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: a FaceNet and a HandNet context are required");
-  if (pose->kp_out != 0) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the first context must hold the pose net");
-  if (face->kp_out != 71) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the face context does not hold FaceNet");
-  if (hand->kp_out != 22) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: the hand context does not hold HandNet");
+  if (!face || !hand) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: a FaceNet and a HandNet context are required");
+  if (pose->kp_out != 0) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_batch: the first context must hold the pose net");
+  if (face->kp_out != 71) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_batch: the face context does not hold FaceNet");
+  if (hand->kp_out != 22) OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_batch: the hand context does not hold HandNet");
   if (pose->precision < 0 || face->precision < 0 || hand->precision < 0)
-    OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_frame: opb_finalize_weights has not been called on every context");
+    OPB_FAIL(pose, OPB_ERR_STATE, "whole_body_batch: opb_finalize_weights has not been called on every context");
   if (face->device != pose->device || hand->device != pose->device)
-    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: the three contexts must be on the same device");
-  if (!img || orig_h <= 0 || orig_w <= 0 || in_h <= 0 || in_w <= 0 || in_h % 8 || in_w % 8 || map_h <= 0 || map_w <= 0)
-    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: bad frame, input or map size");
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: the three contexts must be on the same device");
+  if (n < 1) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: the batch must hold at least one frame");
+  if (!frames || orig_h <= 0 || orig_w <= 0 || in_h <= 0 || in_w <= 0 || in_h % 8 || in_w % 8 || map_h <= 0 || map_w <= 0)
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: bad frame, input or map size");
+  const size_t px = static_cast<size_t>(orig_h) * orig_w;
+  if (static_cast<unsigned long long>(n) * px > (1ull << 31) - 256)
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: more than 2^31 pixels in one batch");
   if (face_net_size <= 0 || face_net_size % 8 || hand_net_size <= 0 || hand_net_size % 8)
-    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: net sizes must be positive multiples of 8");
-  if (!header_out || !persons_out || !n_parts || parts_cap < 0 ||
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: net sizes must be positive multiples of 8");
+  if (!headers_out || !persons_out || !n_parts || !frame_parts || parts_cap < 0 ||
       (parts_cap > 0 && (!parts_out || !face_out || !face_valid || !hand_out || !hand_valid)))
-    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: bad output arguments");
+    OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: bad output arguments");
   *n_parts = 0;
   cudaSetDevice(pose->device);
   const double sx = static_cast<double>(orig_w) / map_w, sy = static_cast<double>(orig_h) / map_h;  // :513-514
   const int cap = pose->prm.max_persons;
-  const size_t rec_b = sizeof(ImageHeader) + sizeof(PersonOut) * static_cast<size_t>(cap);
-  const WbLayout L = wb_layout(cap);
+  const size_t rec_b = static_cast<size_t>(n) * (sizeof(ImageHeader) + sizeof(PersonOut) * static_cast<size_t>(cap));
+  const WbLayout L = wb_layout(cap, n);
   int rc;
-  // (1) one upload of the frame, the device resize and the pipeline of opb_detect_image
+  // (1) one upload of all frames, one device resize of the batch and the pipeline at batch n, the launch sequence of
+  // opb_stream_submit for n frames
   Chain* ch = nullptr;
   PostWs* ws = nullptr;
-  if ((rc = get_chain(pose, 1, in_h, in_w, &ch))) return rc;
-  if ((rc = get_post(pose, 1, map_h, map_w, &ws))) return rc;
+  if ((rc = get_chain(pose, n, in_h, in_w, &ch))) return rc;
+  if ((rc = get_post(pose, n, map_h, map_w, &ws))) return rc;
   WbOut wo;
-  if ((rc = wb_reserve(pose, cap, 0, rec_b + L.tables_end, &wo))) return rc;
-  const size_t in_b = static_cast<size_t>(orig_h) * orig_w * 3;
-  const uint8_t* d_frame = img;
-  if (img_loc == OPB_HOST) {
+  if ((rc = wb_reserve(pose, cap, n, 0, rec_b + L.tables_end, &wo))) return rc;
+  const size_t in_b = px * 3 * n;
+  const uint8_t* d_frames = frames;
+  if (frames_loc == OPB_HOST) {
     if ((rc = ensure_ingest(pose, in_b + 512))) return rc;
-    if ((rc = copy_in(pose, pose->ingest_buf, img, in_b, OPB_HOST))) return rc;
-    d_frame = pose->ingest_buf;
+    if ((rc = copy_in(pose, pose->ingest_buf, frames, in_b, OPB_HOST))) return rc;
+    d_frames = pose->ingest_buf;
   }
-  if ((rc = launch_resize_u8(pose, d_frame, 1, orig_h, orig_w, ch->img_u8, in_h, in_w))) return rc;
+  if ((rc = launch_resize_u8(pose, d_frames, n, orig_h, orig_w, ch->img_u8, in_h, in_w))) return rc;
   ch->img_u8_src = nullptr;
   // (2) inject_* replace the network output, as in opb_detect_batch
-  if ((rc = run_pipeline(pose, ch, ws, 1, in_h, in_w, map_h, map_w, img_len, inject_paf, inject_heat))) return rc;
-  // (3) the crop boxes, then one download of the records and the tables and one synchronisation
-  if ((rc = wb_launch(pose, ws->headers, ws->persons, cap, sx, sy, wo))) return rc;
-  static_assert(sizeof(ImageHeader) % 16 == 0, "the persons follow the header in the record block");
+  if ((rc = run_pipeline(pose, ch, ws, n, in_h, in_w, map_h, map_w, img_len, inject_paf, inject_heat))) return rc;
+  // (3) the crop boxes of every frame in one launch, then one download of the records and the tables and one
+  // synchronisation
+  if ((rc = wb_launch(pose, ws->headers, ws->persons, n, cap, sx, sy, wo))) return rc;
+  static_assert(sizeof(ImageHeader) % 16 == 0, "the persons follow the headers in the record block");
   OPB_CUDA(pose, cudaMemcpyAsync(pose->wb_host, ws->headers, rec_b, cudaMemcpyDeviceToHost, pose->stream));
   OPB_CUDA(pose, cudaMemcpyAsync(pose->wb_host + rec_b, pose->wb_buf, L.tables_end, cudaMemcpyDeviceToHost, pose->stream));
   OPB_CUDA(pose, cudaStreamSynchronize(pose->stream));
   const uint8_t* hb = pose->wb_host;
-  std::memcpy(header_out, hb, sizeof(ImageHeader));
-  std::memcpy(persons_out, hb + sizeof(ImageHeader), sizeof(PersonOut) * static_cast<size_t>(cap));
-  const ImageHeader hd = *reinterpret_cast<const ImageHeader*>(hb);
-  if (hd.status != 0) OPB_FAIL(pose, hd.status, "whole_body_frame: the frame's result carries an error status");
-  const WbCounts cnt = *reinterpret_cast<const WbCounts*>(hb + rec_b + L.counts);
-  if (cnt.status != 0) OPB_FAIL(pose, cnt.status, "whole_body_frame: a crop box edge does not fit int32");
+  const ImageHeader* hds = reinterpret_cast<const ImageHeader*>(hb);
+  std::memcpy(headers_out, hb, sizeof(ImageHeader) * n);
+  std::memcpy(persons_out, hb + sizeof(ImageHeader) * n, sizeof(PersonOut) * static_cast<size_t>(cap) * n);
+  for (int f = 0; f < n; ++f)
+    if (hds[f].status != 0)
+      OPB_FAIL(pose, hds[f].status, "whole_body_batch: frame " + std::to_string(f) + "'s result carries an error status");
+  const WbCounts* cnt = reinterpret_cast<const WbCounts*>(hb + rec_b + L.counts);
+  for (int f = 0; f < n; ++f)
+    if (cnt[f].status != 0)
+      OPB_FAIL(pose, cnt[f].status, "whole_body_batch: a crop box edge of frame " + std::to_string(f) + " does not fit int32");
   const WbCrop* h_face = reinterpret_cast<const WbCrop*>(hb + rec_b + L.face);
   const WbCrop* h_hand = reinterpret_cast<const WbCrop*>(hb + rec_b + L.hand);
   const WbPart* h_parts = reinterpret_cast<const WbPart*>(hb + rec_b + L.parts);
-  *n_parts = cnt.n_parts;
-  if (cnt.n_parts > parts_cap) OPB_FAIL(pose, OPB_ERR_CAPACITY, "whole_body_frame: more parts than parts_cap");
+  long long total = 0;
+  frame_parts[0] = 0;
+  for (int f = 0; f < n; ++f) {
+    total += cnt[f].n_parts;
+    frame_parts[f + 1] = static_cast<int>(std::min<long long>(total, INT32_MAX));
+  }
+  *n_parts = static_cast<int>(std::min<long long>(total, INT32_MAX));
+  if (total > parts_cap) OPB_FAIL(pose, OPB_ERR_CAPACITY, "whole_body_batch: more parts than parts_cap");
+  // the sections of every frame, concatenated frame by frame: face / hand rows run over the whole batch
   std::vector<KpCrop> ftab, htab;
-  if ((rc = wb_kp_table(pose, h_face, cnt.n_face, ftab))) return rc;
-  if ((rc = wb_kp_table(pose, h_hand, cnt.n_hand, htab))) return rc;
-  for (int i = 0; i < cnt.n_parts; ++i) {
-    const WbPart& p = h_parts[i];
-    const WbCrop& b = p.side == WB_FACE ? h_face[p.row] : h_hand[p.row];
-    parts_out[i] = opb_wb_part{p.side == WB_FACE ? OPB_PART_FACE : OPB_PART_HAND, b.left, b.top, b.right, b.bottom,
-                               p.row, p.person, p.side};
+  std::vector<int> face_first(n + 1, 0), hand_first(n + 1, 0);
+  for (int f = 0; f < n; ++f) {
+    const size_t fc = static_cast<size_t>(f) * cap;
+    const int face0 = static_cast<int>(ftab.size()), hand0 = static_cast<int>(htab.size());
+    face_first[f] = face0;
+    hand_first[f] = hand0;
+    if ((rc = wb_kp_table(pose, h_face + fc, cnt[f].n_face, f, ftab))) return rc;
+    if ((rc = wb_kp_table(pose, h_hand + 2 * fc, cnt[f].n_hand, f, htab))) return rc;
+    for (int i = 0; i < cnt[f].n_parts; ++i) {
+      const WbPart& p = h_parts[3 * fc + i];
+      const WbCrop& b = p.side == WB_FACE ? h_face[fc + p.row] : h_hand[2 * fc + p.row];
+      parts_out[frame_parts[f] + i] =
+          opb_wb_part{p.side == WB_FACE ? OPB_PART_FACE : OPB_PART_HAND, b.left, b.top, b.right, b.bottom,
+                      p.row + (p.side == WB_FACE ? face0 : hand0), p.person, p.side};
+    }
   }
-  // (4) FaceNet on the face stream and HandNet on the hand stream, both reading the frame in place; both chains are
-  // enqueued before either is collected, so they overlap
-  if (!ftab.empty() && (rc = kp_enqueue_table(face, d_frame, orig_h, orig_w, ftab, face_net_size))) return rc;
-  if (!htab.empty() && (rc = kp_enqueue_table(hand, d_frame, orig_h, orig_w, htab, hand_net_size))) {
-    cudaStreamSynchronize(face->stream);
-    return rc;
-  }
-  int rc_face = OPB_OK, rc_hand = OPB_OK;
-  if (!ftab.empty()) rc_face = kp_peaks_collect(face, face->kp_ws, ftab, face->kp_out - 1, face_thresh, face_out, face_valid);
-  if (!htab.empty()) rc_hand = kp_peaks_collect(hand, hand->kp_ws, htab, hand->kp_out - 1, hand_thresh, hand_out, hand_valid);
-  if (rc_face) { pose->err = face->err; return rc_face; }
-  if (rc_hand) { pose->err = hand->err; return rc_hand; }
-  if (!picture_out) return OPB_OK;
-  // (5) the picture of opb_draw_whole_body, on the resident frame, with the skeleton from the device records
+  face_first[n] = static_cast<int>(ftab.size());
+  hand_first[n] = static_cast<int>(htab.size());
+  // (4) FaceNet on the face stream and HandNet on the hand stream, both reading the frames in place; both chains are
+  // enqueued before either is collected, so they overlap, and their chunks cross frame boundaries.  The ragged maps of
+  // a call hold every crop at its own size, so frames go through the nets in groups of whole frames whose maps stay
+  // under kWbGroupFloats per net (a group holds at least one frame): a batch needs no more map workspace than the
+  // budget or its largest frame.  Groups after the first start a new chunk sequence.
   const int face_pl = face->kp_out - 1, hand_pl = hand->kp_out - 1;
-  std::vector<int32_t> tab(static_cast<size_t>(cnt.n_parts) * 6);
+  auto area = [](const std::vector<KpCrop>& t, int a, int b) {
+    size_t v = 0;
+    for (int i = a; i < b; ++i) v += static_cast<size_t>(t[i].h) * t[i].w;
+    return v;
+  };
+  for (int g0 = 0; g0 < n;) {
+    size_t ff = area(ftab, face_first[g0], face_first[g0 + 1]) * face_pl;
+    size_t hf = area(htab, hand_first[g0], hand_first[g0 + 1]) * hand_pl;
+    int g1 = g0 + 1;
+    for (; g1 < n; ++g1) {
+      const size_t nf = ff + area(ftab, face_first[g1], face_first[g1 + 1]) * face_pl;
+      const size_t nh = hf + area(htab, hand_first[g1], hand_first[g1 + 1]) * hand_pl;
+      if (nf > kWbGroupFloats || nh > kWbGroupFloats) break;
+      ff = nf;
+      hf = nh;
+    }
+    std::vector<KpCrop> fg(ftab.begin() + face_first[g0], ftab.begin() + face_first[g1]);
+    std::vector<KpCrop> hg(htab.begin() + hand_first[g0], htab.begin() + hand_first[g1]);
+    if (!fg.empty() && (rc = kp_enqueue_table(face, d_frames, orig_h, orig_w, fg, face_net_size))) {
+      pose->err = face->err;
+      cudaGetLastError();
+      return rc;
+    }
+    if (!hg.empty() && (rc = kp_enqueue_table(hand, d_frames, orig_h, orig_w, hg, hand_net_size))) {
+      pose->err = hand->err;
+      cudaGetLastError();
+      cudaStreamSynchronize(face->stream);
+      return rc;
+    }
+    const size_t fr0 = face_first[g0], hr0 = hand_first[g0];
+    int rc_face = OPB_OK, rc_hand = OPB_OK;
+    if (!fg.empty())
+      rc_face = kp_peaks_collect(face, face->kp_ws, fg, face_pl, face_thresh, face_out + fr0 * face_pl * 3,
+                                 face_valid + fr0 * face_pl);
+    if (!hg.empty())
+      rc_hand = kp_peaks_collect(hand, hand->kp_ws, hg, hand_pl, hand_thresh, hand_out + hr0 * hand_pl * 3,
+                                 hand_valid + hr0 * hand_pl);
+    if (rc_face) { pose->err = face->err; return rc_face; }
+    if (rc_hand) { pose->err = hand->err; return rc_hand; }
+    g0 = g1;
+  }
+  if (!pictures_out) return OPB_OK;
+  // (5) the pictures of opb_draw_whole_body on the resident frames, the skeletons from the device records: one table
+  // upload, one records -> poses launch, one raster and one paint launch for all n pictures, one download
+  const int n_all = *n_parts;
+  std::vector<int32_t> tab(static_cast<size_t>(n) * 4 + static_cast<size_t>(n_all) * 6);   // [frames | parts | points]
   std::vector<int32_t> pts;
-  for (int i = 0; i < cnt.n_parts; ++i) {
+  long long n_prim = 0;
+  int total_poses = 0;
+  for (int f = 0; f < n; ++f) {
+    const int n_poses = hds[f].n_peaks == 0 ? 0 : std::min(hds[f].n_persons, cap);
+    const int np = frame_parts[f + 1] - frame_parts[f];
+    const int32_t fr[4] = {static_cast<int32_t>(n_prim), n_poses, frame_parts[f], np};
+    std::copy(fr, fr + 4, tab.begin() + 4 * f);
+    n_prim += static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) + static_cast<long long>(np) * OV_PART_STRIDE;
+    total_poses += n_poses;
+    if (n_prim > (1ll << 30)) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: too many poses / parts to draw");
+  }
+  static_assert(sizeof(OvFrame) == 16, "OvFrame rows are four ints");
+  int32_t* tparts = tab.data() + 4 * n;
+  for (int i = 0; i < n_all; ++i) {
     const opb_wb_part& p = parts_out[i];
     const bool is_face = p.kind == OPB_PART_FACE;
     const int count = is_face ? face_pl : hand_pl;
     const double* o = (is_face ? face_out : hand_out) + static_cast<size_t>(p.row) * count * 3;
     const int32_t* v = (is_face ? face_valid : hand_valid) + static_cast<size_t>(p.row) * count;
     const int32_t row[6] = {p.kind, p.left, p.top, p.right, p.bottom, static_cast<int32_t>(pts.size() / 3)};
-    std::copy(row, row + 6, tab.begin() + 6 * i);
+    std::copy(row, row + 6, tparts + 6 * i);
     for (int k = 0; k < count; ++k) {
       pts.push_back(v[k] ? static_cast<int32_t>(o[3 * k]) : 0);
       pts.push_back(v[k] ? static_cast<int32_t>(o[3 * k + 1]) : 0);
@@ -3209,50 +3291,61 @@ int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint
     }
   }
   const int n_points = static_cast<int>(pts.size() / 3);
-  if ((rc = check_parts(pose, reinterpret_cast<const opb_part*>(tab.data()), cnt.n_parts, pts.data(), n_points))) return rc;
+  if ((rc = check_parts(pose, reinterpret_cast<const opb_part*>(tparts), n_all, pts.data(), n_points))) return rc;
   tab.insert(tab.end(), pts.begin(), pts.end());
-  const int n_poses = hd.n_peaks == 0 ? 0 : hd.n_persons;
-  const size_t px = static_cast<size_t>(orig_h) * orig_w, img_b = (px * 3 + 255) & ~size_t(255);
-  const size_t prio_b = (px * 4 + 255) & ~size_t(255);
-  const size_t poses_b = (static_cast<size_t>(std::max(n_poses, 1)) * OV_JOINTS * 3 * 4 + 255) & ~size_t(255);
+  const size_t img_b = (px * 3 * n + 255) & ~size_t(255), prio_b = (px * 4 * n + 255) & ~size_t(255);
+  const size_t poses_b = (static_cast<size_t>(n) * cap * OV_JOINTS * 3 * 4 + 255) & ~size_t(255);
   const size_t tab_b = (tab.size() * 4 + 255) & ~size_t(255);
-  // scratch: [picture | priority plane | int poses | parts and points | flag]
+  // scratch: [pictures | priority planes | int poses [n][cap] | frames, parts and points | flag]
   if ((rc = ov_reserve(pose, img_b + prio_b + poses_b + tab_b + 256))) return rc;
   uint8_t* d_out = pose->ov_buf;
   unsigned int* d_prio = reinterpret_cast<unsigned int*>(pose->ov_buf + img_b);
   int* d_poses = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b);
   int* d_tab = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b + poses_b);
   int* d_bad = reinterpret_cast<int*>(pose->ov_buf + img_b + prio_b + poses_b + tab_b);
-  if (!tab.empty() && (rc = copy_in(pose, d_tab, tab.data(), tab.size() * 4, OPB_HOST))) return rc;
-  OPB_CUDA(pose, cudaMemsetAsync(d_prio, 0, px * 4, pose->stream));
+  if ((rc = copy_in(pose, d_tab, tab.data(), tab.size() * 4, OPB_HOST))) return rc;
+  OPB_CUDA(pose, cudaMemsetAsync(d_prio, 0, px * 4 * n, pose->stream));
   OPB_CUDA(pose, cudaMemsetAsync(d_bad, 0, 4, pose->stream));
   const OverlayTables tb = overlay_tables(pose);
-  const OvPart* d_parts = reinterpret_cast<const OvPart*>(d_tab);
-  const int* d_points = d_tab + static_cast<size_t>(cnt.n_parts) * 6;
-  if (n_poses > 0) {
+  const OvFrame* d_fr = reinterpret_cast<const OvFrame*>(d_tab);
+  const OvPart* d_parts = reinterpret_cast<const OvPart*>(d_tab + 4 * n);
+  const int* d_points = d_tab + 4 * n + static_cast<size_t>(n_all) * 6;
+  if (total_poses > 0) {
     const int* base = reinterpret_cast<const int*>(ws->persons);
     const int stride = static_cast<int>(sizeof(PersonOut) / 4), off_id = 4, off_x = 4 + OPB_N_JOINTS, off_y = 4 + 2 * OPB_N_JOINTS;
-    overlay_poses_from_records_kernel<<<(n_poses * OV_JOINTS + 127) / 128, 128, 0, pose->stream>>>(
-        base + off_x, base + off_y, base + off_id, stride, n_poses, sx, sy, d_poses);
+    const size_t threads = static_cast<size_t>(n) * cap * OV_JOINTS;
+    overlay_poses_from_records_batch_kernel<<<static_cast<unsigned>((threads + 127) / 128), 128, 0, pose->stream>>>(
+        base + off_x, base + off_y, base + off_id, stride, cap, d_fr, n, sx, sy, d_poses);
     pose->launches++;
   }
-  const long long n_prim = static_cast<long long>(n_poses) * (OV_LIMBS + OV_JOINTS) +
-                           static_cast<long long>(cnt.n_parts) * OV_PART_STRIDE;
   if (n_prim > 0) {
-    overlay_raster_kernel<<<static_cast<unsigned>((n_prim + 63) / 64), 64, 0, pose->stream>>>(
-        d_poses, n_poses, tb, d_prio, orig_h, orig_w, d_bad, d_parts, cnt.n_parts, d_points);
+    overlay_raster_batch_kernel<<<static_cast<unsigned>((n_prim + 63) / 64), 64, 0, pose->stream>>>(
+        d_poses, cap, d_fr, n, static_cast<int>(n_prim), tb, d_prio, orig_h, orig_w, d_bad, d_parts, d_points);
     pose->launches++;
   }
-  overlay_paint_kernel<<<static_cast<unsigned>((px + 255) / 256), 256, 0, pose->stream>>>(
-      d_frame, d_prio, static_cast<int>(px), n_poses, tb, d_out, d_parts, 1);
+  overlay_paint_batch_kernel<<<static_cast<unsigned>((px * n + 255) / 256), 256, 0, pose->stream>>>(
+      d_frames, d_prio, static_cast<int>(px), d_fr, n, tb, d_out, d_parts);
   pose->launches++;
   OPB_CUDA(pose, cudaGetLastError());
   int bad = 0;
   OPB_CUDA(pose, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, pose->stream));
-  if ((rc = copy_out(pose, picture_out, d_out, px * 3, OPB_HOST))) return rc;
+  if ((rc = copy_out(pose, pictures_out, d_out, px * 3 * n, OPB_HOST))) return rc;
   OPB_CUDA(pose, cudaStreamSynchronize(pose->stream));
-  if (bad) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_frame: a joint lies outside the image");
+  if (bad) OPB_FAIL(pose, OPB_ERR_ARG, "whole_body_batch: a joint lies outside the image");
   return OPB_OK;
+}
+
+int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* img, int img_loc, int orig_h,
+                         int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len, const float* inject_paf,
+                         const float* inject_heat, int face_net_size, double face_thresh, int hand_net_size,
+                         double hand_thresh, opb_image_header* header_out, opb_person* persons_out,
+                         opb_wb_part* parts_out, int parts_cap, int* n_parts, double* face_out, int32_t* face_valid,
+                         double* hand_out, int32_t* hand_valid, uint8_t* picture_out) {
+  int frame_parts[2];
+  return opb_whole_body_batch(pose, face, hand, img, img_loc, 1, orig_h, orig_w, in_h, in_w, map_h, map_w, img_len,
+                              inject_paf, inject_heat, face_net_size, face_thresh, hand_net_size, hand_thresh, header_out,
+                              persons_out, parts_out, parts_cap, n_parts, frame_parts, face_out, face_valid, hand_out,
+                              hand_valid, picture_out);
 }
 
 int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, double sx, double sy, double* unit_out,
@@ -3267,13 +3360,13 @@ int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, do
   const size_t rec_b = sizeof(ImageHeader) + sizeof(PersonOut) * static_cast<size_t>(cap);
   WbOut wo;
   int rc;
-  if ((rc = wb_reserve(ctx, cap, rec_b, L.total, &wo))) return rc;
+  if ((rc = wb_reserve(ctx, cap, 1, rec_b, L.total, &wo))) return rc;
   ImageHeader* d_hd = reinterpret_cast<ImageHeader*>(ctx->wb_buf + L.total);
   PersonOut* d_persons = reinterpret_cast<PersonOut*>(ctx->wb_buf + L.total + sizeof(ImageHeader));
   const ImageHeader hd{1, n, 0, 0};
   if ((rc = copy_in(ctx, d_hd, &hd, sizeof(hd), OPB_HOST))) return rc;
   if (n > 0 && (rc = copy_in(ctx, d_persons, persons, sizeof(PersonOut) * n, OPB_HOST))) return rc;
-  if ((rc = wb_launch(ctx, d_hd, d_persons, cap, sx, sy, wo))) return rc;
+  if ((rc = wb_launch(ctx, d_hd, d_persons, 1, cap, sx, sy, wo))) return rc;
   OPB_CUDA(ctx, cudaMemcpyAsync(ctx->wb_host, ctx->wb_buf, L.total, cudaMemcpyDeviceToHost, ctx->stream));
   OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   const uint8_t* hb = ctx->wb_host;
@@ -3290,6 +3383,42 @@ int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, do
     parts_out[2 * i + 1] = parts[i].side;
   }
   *n_parts = cnt.n_parts;
+  return OPB_OK;
+}
+
+int opb_test_whole_body_boxes_batch(opb_ctx* ctx, const opb_image_header* headers, const opb_person* persons, int n,
+                                    int cap, double sx, double sy, int32_t* counts_out, double* unit_out,
+                                    int32_t* boxes_out, int32_t* present_out, opb_crop* face_out, opb_crop* hand_out,
+                                    int32_t* parts_out) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (n < 1 || cap < 1 || static_cast<long long>(n) * cap > (1 << 16) || !headers || !persons || !counts_out ||
+      !unit_out || !boxes_out || !present_out || !face_out || !hand_out || !parts_out || !std::isfinite(sx) ||
+      !std::isfinite(sy))
+    OPB_FAIL(ctx, OPB_ERR_ARG, "test_whole_body_boxes_batch: bad arguments");
+  cudaSetDevice(ctx->device);
+  const size_t c = static_cast<size_t>(n) * cap;
+  const WbLayout L = wb_layout(cap, n);
+  const size_t hd_b = (sizeof(ImageHeader) * n + 255) & ~size_t(255);
+  WbOut wo;
+  int rc;
+  if ((rc = wb_reserve(ctx, cap, n, hd_b + sizeof(PersonOut) * c, L.total, &wo))) return rc;
+  ImageHeader* d_hd = reinterpret_cast<ImageHeader*>(ctx->wb_buf + L.total);
+  PersonOut* d_persons = reinterpret_cast<PersonOut*>(ctx->wb_buf + L.total + hd_b);
+  if ((rc = copy_in(ctx, d_hd, headers, sizeof(ImageHeader) * n, OPB_HOST))) return rc;
+  if ((rc = copy_in(ctx, d_persons, persons, sizeof(PersonOut) * c, OPB_HOST))) return rc;
+  // outputs a frame does not write (error status, no peaks, persons past n_persons) read back as zero
+  OPB_CUDA(ctx, cudaMemsetAsync(ctx->wb_buf, 0, L.total, ctx->stream));
+  if ((rc = wb_launch(ctx, d_hd, d_persons, n, cap, sx, sy, wo))) return rc;
+  OPB_CUDA(ctx, cudaMemcpyAsync(ctx->wb_host, ctx->wb_buf, L.total, cudaMemcpyDeviceToHost, ctx->stream));
+  OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  const uint8_t* hb = ctx->wb_host;
+  std::memcpy(counts_out, hb + L.counts, sizeof(WbCounts) * n);
+  std::memcpy(unit_out, hb + L.unit, sizeof(double) * c);
+  std::memcpy(boxes_out, hb + L.box, sizeof(int) * 12 * c);
+  std::memcpy(present_out, hb + L.present, sizeof(int) * c);
+  std::memcpy(face_out, hb + L.face, sizeof(WbCrop) * c);
+  std::memcpy(hand_out, hb + L.hand, sizeof(WbCrop) * 2 * c);
+  std::memcpy(parts_out, hb + L.parts, sizeof(WbPart) * 3 * c);
   return OPB_OK;
 }
 

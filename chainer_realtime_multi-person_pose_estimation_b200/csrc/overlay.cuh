@@ -314,17 +314,24 @@ __device__ inline void ov_thick_line2(const OvCanvas& cv, int x0, int y0, int x1
 }
 
 // records of the pipeline -> the reference's `poses.round().astype('i')` (:513-514 then :539):
-// x = rint(double(peak x) * sx), y likewise, v = 2 for a present joint; absent joints are (0, 0, 0)
+// x = rint(double(peak x) * sx), y likewise, v = 2 for a present joint; absent joints are (0, 0, 0).  Joint j of
+// record p -> poses row i.
+__device__ __forceinline__ void ov_pose_joint(const int* __restrict__ rec_x, const int* __restrict__ rec_y,
+                                              const int* __restrict__ rec_id, int person_stride_ints, size_t p, int j,
+                                              double sx, double sy, int* __restrict__ poses, size_t i) {
+  const bool has = rec_id[p * person_stride_ints + j] >= 0;
+  poses[3 * i + 0] = has ? __double2int_rn(__dmul_rn(static_cast<double>(rec_x[p * person_stride_ints + j]), sx)) : 0;
+  poses[3 * i + 1] = has ? __double2int_rn(__dmul_rn(static_cast<double>(rec_y[p * person_stride_ints + j]), sy)) : 0;
+  poses[3 * i + 2] = has ? 2 : 0;
+}
+
 __global__ void overlay_poses_from_records_kernel(const int* __restrict__ rec_x, const int* __restrict__ rec_y,
                                                   const int* __restrict__ rec_id, int person_stride_ints, int n_persons,
                                                   double sx, double sy, int* __restrict__ poses) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_persons * OV_JOINTS) return;
   const int p = i / OV_JOINTS, j = i - p * OV_JOINTS;
-  const bool has = rec_id[static_cast<size_t>(p) * person_stride_ints + j] >= 0;
-  poses[3 * i + 0] = has ? __double2int_rn(__dmul_rn(static_cast<double>(rec_x[static_cast<size_t>(p) * person_stride_ints + j]), sx)) : 0;
-  poses[3 * i + 1] = has ? __double2int_rn(__dmul_rn(static_cast<double>(rec_y[static_cast<size_t>(p) * person_stride_ints + j]), sy)) : 0;
-  poses[3 * i + 2] = has ? 2 : 0;
+  ov_pose_joint(rec_x, rec_y, rec_id, person_stride_ints, static_cast<size_t>(p), j, sx, sy, poses, static_cast<size_t>(i));
 }
 
 // primitive j (< OV_PART_STRIDE) of one face / hand part; pts: the part's (x, y, present) rows in crop coordinates
@@ -356,14 +363,13 @@ __device__ inline void ov_part_primitive(const OvCanvas& cv, const OverlayTables
   }
 }
 
-// one thread per potential primitive: [n_poses * 19 limbs | n_poses * 18 joints | n_parts * OV_PART_STRIDE part
-// primitives] in the reference's drawing order.  `bad` is raised when a drawn joint lies outside the image.
-__global__ void overlay_raster_kernel(const int* __restrict__ poses, int n_poses, OverlayTables tb, unsigned int* __restrict__ prio,
-                                      int H, int W, int* __restrict__ bad, const OvPart* __restrict__ parts, int n_parts,
-                                      const int* __restrict__ points) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_limb = n_poses * OV_LIMBS, n_skel = n_limb + n_poses * OV_JOINTS, n_all = n_skel + n_parts * OV_PART_STRIDE;
-  if (i >= n_all) return;
+// primitive i of one picture's index space [n_poses * 19 limbs | n_poses * 18 joints | n_parts * OV_PART_STRIDE part
+// primitives] in the reference's drawing order, drawn with priority i + 1.  `bad` is raised when a drawn joint lies
+// outside the image.
+__device__ inline void ov_raster_primitive(const int* __restrict__ poses, int n_poses, const OverlayTables& tb,
+                                           unsigned int* __restrict__ prio, int H, int W, int* __restrict__ bad,
+                                           const OvPart* __restrict__ parts, const int* __restrict__ points, int i) {
+  const int n_limb = n_poses * OV_LIMBS, n_skel = n_limb + n_poses * OV_JOINTS;
   OvCanvas cv{prio, H, W, static_cast<unsigned int>(i) + 1u};
   if (i < n_limb) {
     const int p = i / OV_LIMBS, l = i - p * OV_LIMBS;
@@ -386,6 +392,61 @@ __global__ void overlay_raster_kernel(const int* __restrict__ poses, int n_poses
   }
 }
 
+// one thread per potential primitive of one picture
+__global__ void overlay_raster_kernel(const int* __restrict__ poses, int n_poses, OverlayTables tb, unsigned int* __restrict__ prio,
+                                      int H, int W, int* __restrict__ bad, const OvPart* __restrict__ parts, int n_parts,
+                                      const int* __restrict__ points) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_poses * (OV_LIMBS + OV_JOINTS) + n_parts * OV_PART_STRIDE) return;
+  ov_raster_primitive(poses, n_poses, tb, prio, H, W, bad, parts, points, i);
+}
+
+// ---- n pictures of equally sized frames in one raster and one paint launch (opb_whole_body_batch) ----
+// Frame f keeps its own 1-based priority index space [limbs | joints | parts] and its own priority plane
+// prio + f * H * W.  Its primitives are prim0 .. prim0 + n_poses * 37 + n_parts * OV_PART_STRIDE - 1 of the launch;
+// its poses start at person f * pose_stride of `poses`, its parts at parts + part0 (first_point indexes the shared points).
+struct OvFrame {
+  int prim0, n_poses, part0, n_parts;
+};
+
+// The frame that owns primitive t: the last of frames[0..n) with prim0 <= t (prim0 ascending, frames[0].prim0 == 0);
+// a frame without primitives shares its prim0 with the next one and is never returned for a t it does not own.
+__device__ __forceinline__ int ov_find_frame(const OvFrame* __restrict__ frames, int n, int t) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (frames[mid].prim0 <= t) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// the records of n_frames frames, max_persons (= cap) each, frame f's persons at f * cap: joint rows of the first
+// frames[f].n_poses persons of every frame go to poses [n_frames][cap][18][3]; grid over n_frames * cap * 18 threads
+__global__ void overlay_poses_from_records_batch_kernel(const int* __restrict__ rec_x, const int* __restrict__ rec_y,
+                                                        const int* __restrict__ rec_id, int person_stride_ints, int cap,
+                                                        const OvFrame* __restrict__ frames, int n_frames, double sx,
+                                                        double sy, int* __restrict__ poses) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<size_t>(n_frames) * cap * OV_JOINTS) return;
+  const size_t p = i / OV_JOINTS;
+  const int j = static_cast<int>(i - p * OV_JOINTS), f = static_cast<int>(p / cap);
+  if (static_cast<int>(p - static_cast<size_t>(f) * cap) >= frames[f].n_poses) return;
+  ov_pose_joint(rec_x, rec_y, rec_id, person_stride_ints, p, j, sx, sy, poses, i);
+}
+
+// one thread per potential primitive of all n_frames pictures (n_prim in all); pose_stride: persons per frame in poses
+__global__ void overlay_raster_batch_kernel(const int* __restrict__ poses, int pose_stride, const OvFrame* __restrict__ frames,
+                                            int n_frames, int n_prim, OverlayTables tb, unsigned int* __restrict__ prio,
+                                            int H, int W, int* __restrict__ bad, const OvPart* __restrict__ parts,
+                                            const int* __restrict__ points) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_prim) return;
+  const int f = ov_find_frame(frames, n_frames, i);
+  const OvFrame fr = frames[f];
+  ov_raster_primitive(poses + static_cast<size_t>(f) * pose_stride * OV_JOINTS * 3, fr.n_poses, tb,
+                      prio + static_cast<size_t>(f) * H * W, H, W, bad, parts + fr.part0, points, i - fr.prim0);
+}
+
 // cv2.addWeighted(a, 0.6, b, 0.4, 0) on uint8: saturate_cast<uchar>(a*0.6f + (b*0.4f + 0.f)) in float32, rounded half
 // to even (the same bits with or without a fused multiply-add for every (a, b) pair)
 __device__ __forceinline__ uint8_t ov_blend(uint8_t a, uint8_t b) {
@@ -396,11 +457,10 @@ __device__ __forceinline__ uint8_t ov_blend(uint8_t a, uint8_t b) {
 
 // canvas = orig_img.copy(), then every covered pixel takes the colour of its last primitive.  blend != 0 (whole-body
 // picture): skeleton pixels take blend(img, skeleton colour) instead; part pixels always take the part's colour.
-__global__ void __launch_bounds__(256)
-overlay_paint_kernel(const uint8_t* __restrict__ img, const unsigned int* __restrict__ prio, int n_pix, int n_poses,
-                     OverlayTables tb, uint8_t* __restrict__ out, const OvPart* __restrict__ parts, int blend) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_pix) return;
+// Pixel i of one picture.
+__device__ __forceinline__ void ov_paint_pixel(const uint8_t* __restrict__ img, const unsigned int* __restrict__ prio,
+                                               int n_poses, const OverlayTables& tb, uint8_t* __restrict__ out,
+                                               const OvPart* __restrict__ parts, int blend, size_t i) {
   const unsigned int t = prio[i];
   uint8_t c0 = img[3 * static_cast<size_t>(i)], c1 = img[3 * static_cast<size_t>(i) + 1], c2 = img[3 * static_cast<size_t>(i) + 2];
   if (t) {
@@ -423,6 +483,26 @@ overlay_paint_kernel(const uint8_t* __restrict__ img, const unsigned int* __rest
   out[3 * static_cast<size_t>(i)] = c0;
   out[3 * static_cast<size_t>(i) + 1] = c1;
   out[3 * static_cast<size_t>(i) + 2] = c2;
+}
+
+__global__ void __launch_bounds__(256)
+overlay_paint_kernel(const uint8_t* __restrict__ img, const unsigned int* __restrict__ prio, int n_pix, int n_poses,
+                     OverlayTables tb, uint8_t* __restrict__ out, const OvPart* __restrict__ parts, int blend) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  ov_paint_pixel(img, prio, n_poses, tb, out, parts, blend, static_cast<size_t>(i));
+}
+
+// n_frames whole-body pictures [n_frames][n_pix] (blend on): a thread finds its frame from its pixel index
+__global__ void __launch_bounds__(256)
+overlay_paint_batch_kernel(const uint8_t* __restrict__ imgs, const unsigned int* __restrict__ prio, int n_pix,
+                           const OvFrame* __restrict__ frames, int n_frames, OverlayTables tb, uint8_t* __restrict__ out,
+                           const OvPart* __restrict__ parts) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<size_t>(n_frames) * n_pix) return;
+  const int f = static_cast<int>(i / static_cast<size_t>(n_pix));
+  const OvFrame fr = frames[f];
+  ov_paint_pixel(imgs, prio, fr.n_poses, tb, out, parts + fr.part0, 1, i);
 }
 
 }  // namespace opb

@@ -159,15 +159,26 @@ __device__ __forceinline__ bool wb_person(const PersonOut& rec, double sx, doubl
   return ok;
 }
 
-// One block of WB_THREADS: persons in chunks of WB_THREADS, a block scan of each chunk's kept faces and hands places
-// them in the demo's order.
+// Grid n, one block of WB_THREADS per frame: block f reads hd[f] and persons[f * cap ..] and writes the frame's
+// section of every output (counts[f]; unit, box, present and the face table from f * cap; the hand table from
+// f * 2 cap; the part list from f * 3 cap), persons in chunks of WB_THREADS, a block scan of each chunk's kept faces
+// and hands placing them in the demo's order.  A frame with an error status or without peaks contributes nothing.
 __global__ void __launch_bounds__(WB_THREADS)
 whole_body_boxes_kernel(const ImageHeader* __restrict__ hd, const PersonOut* __restrict__ persons, int cap, double sx,
                         double sy, WbOut out) {
   __shared__ int scan[2][WB_THREADS];
   __shared__ int base_face, base_hand, bad;
   const int tid = threadIdx.x;
-  const ImageHeader h = *hd;
+  const size_t f = blockIdx.x, fc = f * static_cast<size_t>(cap);
+  persons += fc;
+  out.counts += f;
+  out.unit += fc;
+  out.box += fc * 12;
+  out.present += fc;
+  out.face += fc;
+  out.hand += 2 * fc;
+  out.parts += 3 * fc;
+  const ImageHeader h = hd[f];
   if (h.status != 0) {
     if (tid == 0) *out.counts = WbCounts{h.status, 0, 0, 0};
     return;

@@ -3,6 +3,7 @@
     res = draw_whole_body(img, poses, parts)                      # host: the cv2 calls demo.py makes
     res = draw_whole_body(img, poses, parts, engine=det.engine)   # device: the same pixels, one upload, one download
     poses, scores, parts, owners, res = detect_whole_body(img, pose_detector, face_detector, hand_detector)
+    results = detect_whole_body_batch(frames, pose_detector, face_detector, hand_detector)   # one tuple per frame
 
 `parts` lists (kind, bbox, keypoints) in drawing order -- demo.py's is, person by person, face, left hand, right hand:
 kind "face" (70 keypoints) or "hand" (21), bbox (left, top, right, bottom) as PoseDetector.crop_face / crop_hands
@@ -88,9 +89,9 @@ def detect_whole_body(img, pose_detector, face_detector, hand_detector, draw=Tru
     return _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw)
 
 
-def _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw, inject_paf=None, inject_heat=None):
-    """detect_whole_body with inject_paf / inject_heat: device maps [1,38,H/8,W/8] / [1,19,H/8,W/8] that replace the
-    pose network's output, as in Engine.detect_batch (stick-figure persons for tests and benchmarks)"""
+def _checked_engines(pose_detector, face_detector, hand_detector):
+    """(pose, face, hand) engines; ValueError for a precise PoseDetector, a detector in the wrong slot or detectors on
+    different devices"""
     if getattr(pose_detector, "precise", False):
         raise ValueError("detect_whole_body runs the single-scale path; a precise PoseDetector is not supported")
     pe, fe, he = pose_detector.engine, face_detector.engine, hand_detector.engine
@@ -102,6 +103,25 @@ def _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw, i
         raise ValueError("hand_detector must hold HandNet (22 output channels), got %d" % getattr(he, "kp_channels", 0))
     if not pe.device == fe.device == he.device:
         raise ValueError("the detectors are on different devices (%d, %d, %d)" % (pe.device, fe.device, he.device))
+    return pe, fe, he
+
+
+def _frame_result(pose_detector, header, persons, table, faces, hands, picture, sx, sy):
+    """one frame's (poses, scores, parts, owners, picture) from its records and its rows of the part table"""
+    poses, scores = pose_detector._poses_from_records(header, persons, sx, sy)
+    parts, owners = [], []
+    for r in table:
+        face = int(r["kind"]) == _native.PART_FACE
+        kps = (faces if face else hands)[int(r["row"])]
+        parts.append(("face" if face else "hand", (int(r["left"]), int(r["top"]), int(r["right"]), int(r["bottom"])), kps))
+        owners.append((int(r["person"]), _SIDES[int(r["side"])]))
+    return poses, scores, parts, owners, picture
+
+
+def _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw, inject_paf=None, inject_heat=None):
+    """detect_whole_body with inject_paf / inject_heat: device maps [1,38,H/8,W/8] / [1,19,H/8,W/8] that replace the
+    pose network's output, as in Engine.detect_batch (stick-figure persons for tests and benchmarks)"""
+    pe, fe, he = _checked_engines(pose_detector, face_detector, hand_detector)
     img = np.asarray(img)
     if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
         raise ValueError("img must be a uint8 [H, W, 3] BGR frame, got %s %s" % (img.dtype, img.shape))
@@ -113,11 +133,61 @@ def _detect_whole_body(img, pose_detector, face_detector, hand_detector, draw, i
         params['face_heatmap_peak_thresh'], params["hand_inference_img_size"], params['hand_heatmap_peak_thresh'],
         draw=draw, inject_paf=inject_paf, inject_heat=inject_heat)
     pose_detector._last_scale = (ow / map_w, oh / map_h)
-    poses, scores = pose_detector._poses_from_records(headers[0], persons[0], ow / map_w, oh / map_h)
-    parts, owners = [], []
-    for r in table:
-        face = int(r["kind"]) == _native.PART_FACE
-        kps = (faces if face else hands)[int(r["row"])]
-        parts.append(("face" if face else "hand", (int(r["left"]), int(r["top"]), int(r["right"]), int(r["bottom"])), kps))
-        owners.append((int(r["person"]), _SIDES[int(r["side"])]))
-    return poses, scores, parts, owners, picture
+    return _frame_result(pose_detector, headers[0], persons[0], table, faces, hands, picture, ow / map_w, oh / map_h)
+
+
+def detect_whole_body_batch(frames, pose_detector, face_detector, hand_detector, draw=True):
+    """detect_whole_body for a batch of video frames in one device call (opb_whole_body_batch): all frames through one
+    pose forward at batch N, one crop-box launch, the face crops of all frames through FaceNet and the hand crops
+    through HandNet in shared chunks, and all pictures in one raster and one paint launch.
+    `frames` is a uint8 [N, H, W, 3] array or a sequence of equally sized BGR frames.  Returns a list of N tuples
+    (poses, scores, parts, owners, picture), each what detect_whole_body returns for that frame (with the pose pass at
+    batch N: results equal detect_whole_body's bit for bit where the conv tiles are the same, see DESIGN 4.2); an empty
+    batch returns [] and launches nothing.  ValueError, before anything is launched, for frames of different sizes, a
+    wrong dtype or shape, and the detector errors of detect_whole_body; a frame's result status raises what
+    PoseDetector.detect_batch raises for it.  Afterwards pose_detector.draw_last_result(frames[0]) draws the first
+    frame's skeleton."""
+    return _detect_whole_body_batch(frames, pose_detector, face_detector, hand_detector, draw)
+
+
+def _checked_frames(frames):
+    """frames -> contiguous uint8 [N, H, W, 3]; ValueError for a wrong dtype or shape or frames of different sizes"""
+    if isinstance(frames, np.ndarray):
+        batch = frames
+        if batch.ndim != 4 or batch.shape[3] != 3 or batch.dtype != np.uint8:
+            raise ValueError("frames must be a uint8 [N, H, W, 3] BGR batch, got %s %s" % (batch.dtype, batch.shape))
+    else:
+        items = [np.asarray(f) for f in frames]
+        for i, f in enumerate(items):
+            if f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3:
+                raise ValueError("frame %d must be a uint8 [H, W, 3] BGR frame, got %s %s" % (i, f.dtype, f.shape))
+            if f.shape != items[0].shape:
+                raise ValueError("frame %d is %s, frame 0 is %s: a batch holds equally sized frames"
+                                 % (i, f.shape, items[0].shape))
+        if not items:
+            return np.zeros((0, 0, 0, 3), np.uint8)
+        batch = np.stack(items)
+    if batch.shape[0] and (batch.shape[1] == 0 or batch.shape[2] == 0):
+        raise ValueError("frames must not be empty images, got %s" % (batch.shape,))
+    return np.ascontiguousarray(batch)
+
+
+def _detect_whole_body_batch(frames, pose_detector, face_detector, hand_detector, draw, inject_paf=None,
+                             inject_heat=None):
+    """detect_whole_body_batch with inject_paf / inject_heat: device maps [N,38,H/8,W/8] / [N,19,H/8,W/8] that replace
+    the pose network's output, as in Engine.detect_batch (stick-figure persons for tests and benchmarks)"""
+    pe, fe, he = _checked_engines(pose_detector, face_detector, hand_detector)
+    frames = _checked_frames(frames)
+    if len(frames) == 0:
+        return []
+    oh, ow = frames.shape[1:3]
+    in_w, in_h = pose_detector.compute_optimal_size(frames[0], params['inference_img_size'])
+    map_w, map_h = pose_detector.compute_optimal_size(frames[0], params['heatmap_size'])
+    headers, persons, table, frame_parts, faces, hands, pictures = pe.whole_body_batch(
+        fe, he, frames, in_h, in_w, map_h, map_w, map_w, params["face_inference_img_size"],
+        params['face_heatmap_peak_thresh'], params["hand_inference_img_size"], params['hand_heatmap_peak_thresh'],
+        draw=draw, inject_paf=inject_paf, inject_heat=inject_heat)
+    pose_detector._last_scale = (ow / map_w, oh / map_h)
+    return [_frame_result(pose_detector, headers[f], persons[f], table[frame_parts[f]:frame_parts[f + 1]], faces, hands,
+                          None if pictures is None else pictures[f], ow / map_w, oh / map_h)
+            for f in range(len(frames))]

@@ -371,6 +371,36 @@ int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint
                          double hand_thresh, opb_image_header* header_out, opb_person* persons_out,
                          opb_wb_part* parts_out, int parts_cap, int* n_parts, double* face_out, int32_t* face_valid,
                          double* hand_out, int32_t* hand_valid, uint8_t* picture_out);
+/* opb_whole_body_batch: opb_whole_body_frame for n >= 1 equally sized BGR frames [n, orig_h, orig_w, 3] (host, or
+ * read in place with OPB_DEVICE); opb_whole_body_frame is its n = 1 case.  inject_paf / inject_heat are
+ * [n, 38|19, in_h/8, in_w/8].  Per call:
+ *   1. one upload of all frames, one device resize of the batch and the pipeline at batch n (the launch sequence of
+ *      opb_detect_batch / opb_stream_submit for n frames);
+ *   2. one launch of the crop-box kernel for all frames (one block per frame), then one download of the records and
+ *      the box tables and one synchronisation;
+ *   3. the face crops of all frames, concatenated frame by frame, through FaceNet on the face context's stream and the
+ *      hand crops likewise through HandNet on the hand context's stream, both enqueued before either is collected;
+ *      forward chunks (full chunks of 16, then the remainder rounded up to a power of two) cross frame boundaries.
+ *      Frames go through the nets in groups of whole frames whose crop maps stay under 2^30 floats per net (at least
+ *      one frame per group), so that the map workspace stays bounded; each group has its own chunks and download;
+ *   4. with pictures_out != NULL: one table upload, at most one records -> poses launch, one raster and one paint
+ *      launch for all n pictures, then one download and one synchronisation.
+ * Outputs: headers_out [n] and persons_out [n][max_persons] as opb_stream_collect returns them; parts_out [parts_cap]
+ * (person counts within its frame, row indexes the batch-wide face / hand tables), *n_parts; frame_parts [n + 1]
+ * prefix offsets: frame f owns parts frame_parts[f] .. frame_parts[f+1] - 1, in the demo's order within the frame;
+ * face_out / face_valid / hand_out / hand_valid as opb_whole_body_frame with rows over the whole batch;
+ * pictures_out [n, orig_h, orig_w, 3] host.  The pose context holds the batch's result (opb_draw_last_result with
+ * image_index f).  Errors as opb_whole_body_frame, all checked before anything is enqueued, plus OPB_ERR_ARG for
+ * n < 1; the record status of the first frame that carries one is returned after headers_out and persons_out are
+ * written; OPB_ERR_UNSUPPORTED for a box edge beyond int32; OPB_ERR_CAPACITY when the parts of the batch exceed
+ * parts_cap (*n_parts holds the count). */
+int opb_whole_body_batch(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint8_t* frames, int frames_loc, int n,
+                         int orig_h, int orig_w, int in_h, int in_w, int map_h, int map_w, double img_len,
+                         const float* inject_paf, const float* inject_heat, int face_net_size, double face_thresh,
+                         int hand_net_size, double hand_thresh, opb_image_header* headers_out, opb_person* persons_out,
+                         opb_wb_part* parts_out, int parts_cap, int* n_parts, int* frame_parts /* [n + 1] */,
+                         double* face_out, int32_t* face_valid, double* hand_out, int32_t* hand_valid,
+                         uint8_t* pictures_out);
 /* Test hook: the crop-box kernel of opb_whole_body_frame on n host person records (all persons of one image).
  *   unit_out [n] float64 unit lengths (NaN without a positive limb), boxes_out [n][3][4] (face, left hand, right hand:
  *   left, top, right, bottom), present_out [n] (bit k: box k exists -- its joint is present and the unit length is
@@ -378,6 +408,17 @@ int opb_whole_body_frame(opb_ctx* pose, opb_ctx* face, opb_ctx* hand, const uint
  *   *n_parts.  OPB_ERR_UNSUPPORTED when a box edge does not fit int32. */
 int opb_test_whole_body_boxes(opb_ctx* ctx, const opb_person* persons, int n, double sx, double sy, double* unit_out,
                               int32_t* boxes_out, int32_t* present_out, int32_t* parts_out, int* n_parts);
+/* Test hook: the crop-box kernel of opb_whole_body_batch on the host records of n frames, headers [n] and
+ *   persons [n][cap] (n * cap <= 65536), in one launch.  Per frame f: counts_out [n][4] (status, n_face, n_hand,
+ *   n_parts: a record status error or OPB_ERR_UNSUPPORTED for a box edge beyond int32 is reported here, per frame),
+ *   and the frame's sections unit_out [n][cap], boxes_out [n][cap][3][4], present_out [n][cap] as
+ *   opb_test_whole_body_boxes, face_out [n][cap] and hand_out [n][2 cap] (the compacted crop tables, flip = 1 for
+ *   left hands), parts_out [n][3 cap][4] (side, person, row into the frame's face or hand table, 0).  Entries a frame
+ *   does not write are zero. */
+int opb_test_whole_body_boxes_batch(opb_ctx* ctx, const opb_image_header* headers, const opb_person* persons, int n,
+                                    int cap, double sx, double sy, int32_t* counts_out, double* unit_out,
+                                    int32_t* boxes_out, int32_t* present_out, opb_crop* face_out, opb_crop* hand_out,
+                                    int32_t* parts_out);
 
 /* device pointers of the last opb_detect_batch outputs/intermediates (valid until the next
  * call with a different shape): 0 paf_lo, 1 heat_lo, 2 pafs (full-res), 3 heatmaps (full-res),
