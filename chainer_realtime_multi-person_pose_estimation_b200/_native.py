@@ -49,6 +49,10 @@ CONV_RECORD_DTYPE = np.dtype([("tag", "S32"), ("wkey", "S48", (2,))] + [(f, "<i4
     "ks", "bn", "drain", "comp", "n_problems", "grid", "shared_in", "reserved")] + [
     ("prob", CONV_PROBLEM_DTYPE, (2,))])                                                              # opb_conv_record
 assert CONV_PROBLEM_DTYPE.itemsize == 72 and CONV_RECORD_DTYPE.itemsize == 304
+KP_STAGE_CROP_DTYPE = np.dtype([(f, "<i4") for f in (
+    "left", "top", "right", "bottom", "flip", "frame", "vh", "vw")])                                 # opb_kp_stage_crop
+CHANNEL_MAX_DTYPE = np.dtype([("value", "<f4"), ("count", "<i4"), ("key0", "<i4"), ("key1", "<i4")])  # opb_channel_max
+assert KP_STAGE_CROP_DTYPE.itemsize == 32 and CHANNEL_MAX_DTYPE.itemsize == 16
 
 
 def crop_table(bboxes, flips=None):
@@ -149,6 +153,10 @@ _SIGNATURES = {
     "opb_test_chain_convs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
     "opb_test_chain_conv_run": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "opb_test_keypoint_stages": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                           C.c_int, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_size_t,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     "opb_cascade_load": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "opb_cascade_detect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
@@ -873,3 +881,34 @@ class Engine(object):
         for a in arrs:
             assert a is None or (isinstance(a, np.ndarray) and a.flags.c_contiguous)
         self._check(self.lib.opb_test_chain_conv_run(self.ctx, int(n), int(h), int(w), int(index), *map(_ptr, arrs)))
+
+    def test_keypoint_stages(self, frames, crops, net_size, planes, maps, thresh, tail=4096):
+        """Test hook: the face / hand crop pass (opb_test_keypoint_stages) on frames uint8 [F,H,W,3], crop rows
+        (KP_STAGE_CROP_DTYPE, or (left, top, right, bottom, flip, frame, vh, vw) tuples) and injected maps float32
+        [n][planes + 1][net/8][net/8].  Every output holds `tail` elements past its size.  Returns a dict: sizes
+        (canvas bytes, map floats, records), canvas uint8, up / tmp / smooth float32, records (CHANNEL_MAX_DTYPE),
+        out float64 [n, planes, 3], valid int32 [n, planes] and keypoints (one keypoint list per crop)."""
+        fr = np.ascontiguousarray(frames, np.uint8)
+        rows = np.ascontiguousarray(np.array([tuple(r) for r in crops], KP_STAGE_CROP_DTYPE))
+        mp = np.ascontiguousarray(maps, np.float32)
+        n_frames, fh, fw, _ = fr.shape
+        n = len(rows)
+        sizes = np.zeros(3, np.int64)
+
+        def call(canvas, cc, up, tmp, smooth, mc, rec, rc_, out, valid):
+            return self.lib.opb_test_keypoint_stages(self.ctx, _ptr(fr), n_frames, fh, fw, _ptr(rows), n, int(net_size),
+                                                     int(planes), _ptr(mp), float(thresh), _ptr(canvas), cc, _ptr(up),
+                                                     _ptr(tmp), _ptr(smooth), mc, _ptr(rec), rc_, _ptr(out),
+                                                     _ptr(valid), _ptr(sizes))
+        rc = call(None, 0, None, None, None, 0, None, 0, None, None)
+        if rc != ERR_CAPACITY:
+            self._check(rc)
+        cb, nf, nr = (int(v) + tail for v in sizes)
+        canvas = np.empty(cb, np.uint8)
+        up, tmp, smooth = (np.empty(nf, np.float32) for _ in range(3))
+        records = np.empty(nr, CHANNEL_MAX_DTYPE)
+        out = np.empty((n, planes, 3), np.float64)
+        valid = np.empty((n, planes), np.int32)
+        self._check(call(canvas, cb, up, tmp, smooth, nf, records, nr, out, valid))
+        return dict(sizes=tuple(int(v) for v in sizes), canvas=canvas, up=up, tmp=tmp, smooth=smooth, records=records,
+                    out=out, valid=valid, keypoints=[self._keypoint_list(o, v) for o, v in zip(out, valid)])

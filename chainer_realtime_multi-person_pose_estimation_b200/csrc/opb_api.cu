@@ -2493,6 +2493,50 @@ static int kp_chunk_slots(int remaining) {
   return p;
 }
 
+// Fills in cv2.resize's inverse scales (canvas -> net_size, as launch_resize_u8 forms them) and the ragged layout of
+// `table` (top, left, h, w, flip, vh, vw, frame set).  *tiles: the table's 32x8 tiles; *floats: its maps of `planes`.
+static int kp_prepare_table(opb_ctx* ctx, std::vector<KpCrop>& table, int net_size, int planes, int* tiles,
+                            size_t* floats) {
+  for (KpCrop& c : table) {
+    c.sx = 1.0 / (static_cast<double>(net_size) / c.w);
+    c.sy = 1.0 / (static_cast<double>(net_size) / c.h);
+  }
+  long long t = 0;
+  kp_layout(table, planes, &t, floats);
+  if (t > (1 << 30) || *floats / planes > (1ull << 31)) OPB_FAIL(ctx, OPB_ERR_ARG, "crops too large for one call");
+  *tiles = static_cast<int>(t);
+  return OPB_OK;
+}
+
+// crop_image + flip + cv2.resize(crop, (net, net)) straight from the frames (face_detector.py:31) of the nc crops at
+// d_crops (device table) into dst [slots][net][net][3]; the padding slots nc..slots-1 are zeroed.
+static int kp_canvas_enqueue(opb_ctx* ctx, const uint8_t* d_frames, int frame_h, int frame_w, const KpCrop* d_crops,
+                             int nc, int slots, uint8_t* dst, int net_size) {
+  dim3 rgrid((net_size + 31) / 32, (net_size + 7) / 8, slots);
+  crop_resize_linear_u8_kernel<<<rgrid, dim3(32, 8), 0, ctx->stream>>>(d_frames, frame_h, frame_w, d_crops, nc, dst,
+                                                                       net_size);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  return OPB_OK;
+}
+
+// F.resize_images(hs[-1], (crop_h, crop_w)) (face_detector.py:38) of the chunk table[first, first + nc): slot i of the
+// chunk reads planes [0, planes) of heat_lo + i * kp_out * h8 * h8 (channel `planes` and up, the background, are never
+// read) and writes crop first + i's ragged maps in `up`.  d_crops holds `table` on the device.
+static int kp_upsample_enqueue(opb_ctx* ctx, const float* heat_lo, int kp_out, int planes, int h8,
+                               const std::vector<KpCrop>& table, const KpCrop* d_crops, int first, int nc, int tiles,
+                               float* up) {
+  const int n = static_cast<int>(table.size());
+  const int tile_end = first + nc < n ? table[first + nc].tile0 : tiles;
+  const int ppb = 19;
+  dim3 ugrid(tile_end - table[first].tile0, (planes + ppb - 1) / ppb);
+  upsample_bilinear_ac_ragged_kernel<<<ugrid, dim3(32, 8), 0, ctx->stream>>>(
+      heat_lo, static_cast<size_t>(kp_out) * h8 * h8, planes, h8, h8, d_crops + first, nc, table[first].tile0, up, ppb);
+  ctx->launches++;
+  OPB_CUDA(ctx, cudaGetLastError());
+  return OPB_OK;
+}
+
 // Crops of `table` (top, left, h, w, flip, vh, vw set) of a frame already on the device, through FaceNet / HandNet in
 // chunks of kp_chunk_slots: one crop-table upload, then per chunk a crop + resize launch, the chain and a ragged
 // upsample; then kp_peaks_enqueue.  Nothing waits: kp_peaks_collect(ctx, ctx->kp_ws, table, ...) collects the result.
@@ -2500,17 +2544,9 @@ static int kp_enqueue_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, i
                             int net_size) {
   const int n = static_cast<int>(table.size());
   const int planes = ctx->kp_out - 1;              // the last channel is background (face_detector.py:59)
-  for (KpCrop& c : table) {
-    // cv2.resize's inverse scales, as launch_resize_u8 forms them
-    c.sx = 1.0 / (static_cast<double>(net_size) / c.w);
-    c.sy = 1.0 / (static_cast<double>(net_size) / c.h);
-  }
-  long long t = 0;
+  int tiles = 0, rc;
   size_t floats = 0;
-  kp_layout(table, planes, &t, &floats);
-  if (t > (1 << 30) || floats / planes > (1ull << 31)) OPB_FAIL(ctx, OPB_ERR_ARG, "crops too large for one call");
-  const int tiles = static_cast<int>(t);
-  int rc;
+  if ((rc = kp_prepare_table(ctx, table, net_size, planes, &tiles, &floats))) return rc;
   KpWs* ws = nullptr;
   if ((rc = kp_workspace(ctx, floats, planes * n, n, &ws))) return rc;
   OPB_CUDA(ctx, cudaMemcpyAsync(ws->crops, table.data(), sizeof(KpCrop) * n, cudaMemcpyHostToDevice, ctx->stream));
@@ -2518,23 +2554,13 @@ static int kp_enqueue_table(opb_ctx* ctx, const uint8_t* d_frame, int frame_h, i
     const int slots = kp_chunk_slots(n - first), nc = std::min(slots, n - first);
     Chain* ch = nullptr;
     if ((rc = get_chain(ctx, slots, net_size, net_size, &ch))) return rc;
-    // crop_image + flip + cv2.resize(crop, (net, net)) straight from the frame (face_detector.py:31); padding slots zeroed
-    dim3 rgrid((net_size + 31) / 32, (net_size + 7) / 8, slots);
-    crop_resize_linear_u8_kernel<<<rgrid, dim3(32, 8), 0, ctx->stream>>>(d_frame, frame_h, frame_w, ws->crops + first, nc,
-                                                                         ch->img_u8, net_size);
-    ctx->launches++;
-    OPB_CUDA(ctx, cudaGetLastError());
+    if ((rc = kp_canvas_enqueue(ctx, d_frame, frame_h, frame_w, ws->crops + first, nc, slots, ch->img_u8, net_size)))
+      return rc;
     ch->img_u8_src = nullptr;
     if ((rc = run_chain(ctx, ch, true))) return rc;
-    // F.resize_images(hs[-1], (crop_h, crop_w)) of every crop of the chunk (face_detector.py:38)
-    const int h8 = net_size / 8, tile_end = first + nc < n ? table[first + nc].tile0 : tiles;
-    const int ppb = 19;
-    dim3 ugrid(tile_end - table[first].tile0, (planes + ppb - 1) / ppb);
-    upsample_bilinear_ac_ragged_kernel<<<ugrid, dim3(32, 8), 0, ctx->stream>>>(
-        ch->heat_lo, static_cast<size_t>(ctx->kp_out) * h8 * h8, planes, h8, h8, ws->crops + first, nc,
-        table[first].tile0, ws->up, ppb);
-    ctx->launches++;
-    OPB_CUDA(ctx, cudaGetLastError());
+    if ((rc = kp_upsample_enqueue(ctx, ch->heat_lo, ctx->kp_out, planes, net_size / 8, table, ws->crops, first, nc,
+                                  tiles, ws->up)))
+      return rc;
     first += nc;
   }
   return kp_peaks_enqueue(ctx, ws, table, planes, tiles);
@@ -3710,6 +3736,107 @@ int opb_test_chain_conv_run(opb_ctx* ctx, int n, int h, int w, int index, const 
     if (rec[p].out32) OPB_CUDA(ctx, cudaMemcpyAsync(o32[p], rec[p].out32, planes_bytes(p), cudaMemcpyDeviceToHost, ctx->stream));
   OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return OPB_OK;
+}
+
+static_assert(sizeof(opb_kp_stage_crop) == 32, "opb_kp_stage_crop size");
+static_assert(sizeof(opb_channel_max) == sizeof(ChannelMax), "opb_channel_max mirrors ChannelMax");
+
+int opb_test_keypoint_stages(opb_ctx* ctx, const uint8_t* frames, int n_frames, int frame_h, int frame_w,
+                             const opb_kp_stage_crop* crops, int n, int net_size, int planes, const float* maps,
+                             double thresh, uint8_t* canvas_out, size_t canvas_cap, float* up_out, float* tmp_out,
+                             float* smooth_out, size_t map_cap, opb_channel_max* records_out, size_t records_cap,
+                             double* out, int32_t* valid, int64_t* sizes_out) {
+  if (!ctx) return OPB_ERR_ARG;
+  if (!frames || !crops || !maps || !sizes_out) OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: missing input");
+  if (n < 1 || n > 65535 || n_frames < 1 || frame_h <= 0 || frame_w <= 0)
+    OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: bad crop count or frame size");
+  if (net_size < 16 || net_size > 4096 || net_size % 8)
+    OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: net_size must be a multiple of 8 in [16, 4096]");
+  if (planes < 1 || planes > 1024) OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: planes must be in [1, 1024]");
+  std::vector<KpCrop> table(n);
+  for (int i = 0; i < n; ++i) {
+    const opb_kp_stage_crop& b = crops[i];
+    const long long w = static_cast<long long>(b.right) - b.left, h = static_cast<long long>(b.bottom) - b.top;
+    if (w <= 0 || h <= 0 || w > (1 << 20) || h > (1 << 20) || (b.flip != 0 && b.flip != 1) || b.frame < 0 ||
+        b.frame >= n_frames || b.vh < 0 || b.vh > h || b.vw < 0 || b.vw > w)
+      OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: bad crop row " + std::to_string(i));
+    KpCrop& c = table[i];
+    c.top = b.top; c.left = b.left; c.h = static_cast<int>(h); c.w = static_cast<int>(w); c.flip = b.flip;
+    c.vh = b.vh; c.vw = b.vw; c.frame = b.frame;
+  }
+  int tiles = 0, rc;
+  size_t floats = 0;
+  if ((rc = kp_prepare_table(ctx, table, net_size, planes, &tiles, &floats))) return rc;
+  size_t slots_total = 0;
+  for (int first = 0; first < n; first += std::min(kp_chunk_slots(n - first), n - first))
+    slots_total += kp_chunk_slots(n - first);
+  const size_t canvas_b = slots_total * net_size * net_size * 3, records = static_cast<size_t>(n) * planes;
+  sizes_out[0] = static_cast<int64_t>(canvas_b);
+  sizes_out[1] = static_cast<int64_t>(floats);
+  sizes_out[2] = static_cast<int64_t>(records);
+  if (canvas_cap < canvas_b || map_cap < floats || records_cap < records)
+    OPB_FAIL(ctx, OPB_ERR_CAPACITY, "test_keypoint_stages: output capacity below the sizes in sizes_out");
+  if (!canvas_out || !up_out || !tmp_out || !smooth_out || !records_out || !out || !valid)
+    OPB_FAIL(ctx, OPB_ERR_ARG, "test_keypoint_stages: missing output");
+  cudaSetDevice(ctx->device);
+  const int h8 = net_size / 8;
+  const size_t frame_b = static_cast<size_t>(n_frames) * frame_h * frame_w * 3;
+  const size_t maps_in = static_cast<size_t>(n) * (planes + 1) * h8 * h8;
+  // sentinels: a NaN bit pattern in every 32-bit word of the float and record buffers, 0xA5 in every canvas byte
+  const uint32_t kWord = 0x7FA5A5A5u;
+  std::vector<uint32_t> fill(std::max(map_cap, records_cap * 4), kWord);
+  std::vector<void*> allocs;
+  uint8_t *d_frames = nullptr, *d_canvas = nullptr;
+  float *d_maps = nullptr, *d_up = nullptr, *d_tmp = nullptr;
+  ChannelMax* d_res = nullptr;
+  KpCrop* d_crops = nullptr;
+  auto run = [&]() -> int {
+    int r;
+    if ((r = dev_alloc(ctx, &d_frames, frame_b, allocs, false)) || (r = dev_alloc(ctx, &d_canvas, canvas_cap, allocs, false)) ||
+        (r = dev_alloc(ctx, &d_maps, maps_in, allocs, false)) || (r = dev_alloc(ctx, &d_up, map_cap, allocs, false)) ||
+        (r = dev_alloc(ctx, &d_tmp, map_cap, allocs, false)) || (r = dev_alloc(ctx, &d_res, records_cap, allocs, false)) ||
+        (r = dev_alloc(ctx, &d_crops, table.size(), allocs, false)))
+      return r;
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_frames, frames, frame_b, cudaMemcpyHostToDevice, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_maps, maps, maps_in * 4, cudaMemcpyHostToDevice, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_crops, table.data(), sizeof(KpCrop) * n, cudaMemcpyHostToDevice, ctx->stream));
+    OPB_CUDA(ctx, cudaMemsetAsync(d_canvas, 0xA5, canvas_cap, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_up, fill.data(), map_cap * 4, cudaMemcpyHostToDevice, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_tmp, fill.data(), map_cap * 4, cudaMemcpyHostToDevice, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(d_res, fill.data(), sizeof(ChannelMax) * records_cap, cudaMemcpyHostToDevice, ctx->stream));
+    // the chunks of kp_enqueue_table, with the injected maps in place of each chunk's network output
+    size_t slot0 = 0;
+    for (int first = 0; first < n;) {
+      const int slots = kp_chunk_slots(n - first), nc = std::min(slots, n - first);
+      if ((r = kp_canvas_enqueue(ctx, d_frames, frame_h, frame_w, d_crops + first, nc, slots,
+                                 d_canvas + slot0 * net_size * net_size * 3, net_size)))
+        return r;
+      if ((r = kp_upsample_enqueue(ctx, d_maps + static_cast<size_t>(first) * (planes + 1) * h8 * h8, planes + 1, planes,
+                                   h8, table, d_crops, first, nc, tiles, d_up)))
+        return r;
+      slot0 += slots;
+      first += nc;
+    }
+    OPB_CUDA(ctx, cudaMemcpyAsync(up_out, d_up, map_cap * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    KpWs ws;
+    ws.up = d_up; ws.tmp = d_tmp; ws.res = d_res; ws.crops = d_crops;
+    ws.h_res = reinterpret_cast<ChannelMax*>(records_out);
+    if ((r = kp_peaks_enqueue(ctx, &ws, table, planes, tiles))) return r;
+    OPB_CUDA(ctx, cudaMemcpyAsync(records_out + records, d_res + records, sizeof(ChannelMax) * (records_cap - records),
+                                  cudaMemcpyDeviceToHost, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(canvas_out, d_canvas, canvas_cap, cudaMemcpyDeviceToHost, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(tmp_out, d_tmp, map_cap * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    OPB_CUDA(ctx, cudaMemcpyAsync(smooth_out, d_up, map_cap * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    OPB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int i = 0; i < n; ++i)
+      kp_records_to_keypoints(ws.h_res + static_cast<size_t>(i) * planes, planes, table[i].w, thresh,
+                              out + static_cast<size_t>(i) * planes * 3, valid + static_cast<size_t>(i) * planes);
+    return OPB_OK;
+  };
+  rc = run();
+  cudaStreamSynchronize(ctx->stream);
+  free_all(allocs);
+  return rc;
 }
 
 }  // extern "C"

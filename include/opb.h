@@ -511,6 +511,36 @@ int opb_test_chain_convs(opb_ctx* ctx, int n, int h, int w, opb_conv_record* out
 int opb_test_chain_conv_run(opb_ctx* ctx, int n, int h, int w, int index, const void* in0, const void* in1,
                             void* out_io, float* out32_0, float* out32_1);
 
+/* One crop of opb_test_keypoint_stages: canvas (bottom-top) x (right-left) at (left, top) of frame `frame`, mirrored
+ * when flip = 1; canvas pixels at y >= vh or x >= vw (unmirrored) are zero (vh = h, vw = w: crop_image; smaller: the
+ * zero-padded squares of opb_face_detect_frame).                                                                    */
+typedef struct opb_kp_stage_crop {
+  int32_t left, top, right, bottom, flip, frame, vh, vw;
+} opb_kp_stage_crop;
+typedef struct opb_channel_max {      /* the arg-max record of one (crop, plane)                                   */
+  float value;                        /* maximum of the smoothed map                                              */
+  int32_t count;                      /* pixels equal to it                                                       */
+  int32_t key0, key1;                 /* row-major index of the first / second of them in the (mirrored) map; key1 = -1
+                                         when count < 2                                                           */
+} opb_channel_max;
+/* The face / hand crop pass of opb_keypoints_detect_crops on its own, with injected network maps instead of a
+ * network (no weights needed): frames [n_frames][frame_h][frame_w][3] uint8, maps [n][planes + 1][net/8][net/8]
+ * float32 (channel `planes` is the background: it sits in each slot's stride and is never read).  The same crop
+ * table, chunks (kp_chunk_slots, padding slots included), crop-resize, ragged upsample, two smoothing passes and
+ * arg-max launches as the product.  sizes_out[3] = canvas bytes (16-slot chunks, then a power of two, each slot
+ * net x net x 3), ragged map floats (sum of planes * h * w) and records (n * planes).  Outputs, each with the caller's
+ * capacity (>= those sizes, else OPB_ERR_CAPACITY before anything runs): canvas_out every slot's canvas; up_out the
+ * ragged upsampled maps; tmp_out after the axis-0 pass; smooth_out the smoothed maps; records_out [n][planes];
+ * out / valid [n][planes][3] / [n][planes] as opb_keypoints_detect_crops.  Device buffers are filled before the
+ * launches with 0x7FA5A5A5 in every 32-bit word (float maps, records) and 0xA5 in every canvas byte, and read back
+ * to the full capacity.  OPB_ERR_ARG (nothing enqueued) for a bad crop row, planes outside [1, 1024], net_size not
+ * a multiple of 8 in [16, 4096] or a frame index outside [0, n_frames).                                            */
+int opb_test_keypoint_stages(opb_ctx* ctx, const uint8_t* frames, int n_frames, int frame_h, int frame_w,
+                             const opb_kp_stage_crop* crops, int n, int net_size, int planes, const float* maps,
+                             double thresh, uint8_t* canvas_out, size_t canvas_cap, float* up_out, float* tmp_out,
+                             float* smooth_out, size_t map_cap, opb_channel_max* records_out, size_t records_cap,
+                             double* out, int32_t* valid, int64_t* sizes_out);
+
 #ifdef __cplusplus
 }
 #endif
